@@ -2701,6 +2701,11 @@ size_t mvp_debug_tileclk_offset(const mvp_shape *shape) {
     return make_layout(*shape).tileclk;
 }
 
+size_t mvp_debug_heavy_offset(const mvp_shape *shape) {
+    if (!shape || check_shape(*shape) != MVP_OK) return 0;
+    return make_layout(*shape).heavycnt;
+}
+
 int mvp_forward_launch_count(uint32_t flags) { return (flags & MVP_FLAG_ACCEL_VALID) ? 2 : 6; }   // + 2 ordering kernels for small launches
 int mvp_backward_launch_count(uint32_t flags) { return (flags & MVP_FLAG_ACCEL_VALID) ? 2 : 6; }
 

@@ -80,7 +80,8 @@ EXPORTS = ("mvp_abi_version", "mvp_build_config", "mvp_error_string", "mvp_works
            "mvp_raymarch_forward",
            "mvp_raymarch_backward", "mvp_compute_raydirs", "mvp_forward_launch_count", "mvp_backward_launch_count",
            "mvp_composite_forward", "mvp_composite_backward", "mvp_assemble_payload_forward",
-           "mvp_assemble_payload_backward", "mvp_debug_saved_tiles", "mvp_debug_tileclk_offset", "mvp_compute_morton",
+           "mvp_assemble_payload_backward", "mvp_debug_saved_tiles", "mvp_debug_tileclk_offset", "mvp_debug_heavy_offset",
+           "mvp_compute_morton",
            "mvp_expand_views", "mvp_sum_views")
 
 
@@ -130,6 +131,8 @@ def _load():
     lib.mvp_assemble_payload_forward.argtypes = [ctypes.c_int32] * 4 + [c_f] * 2 + [ctypes.c_float] * 2 + [c_f] * 2
     lib.mvp_assemble_payload_backward.restype = ctypes.c_int
     lib.mvp_assemble_payload_backward.argtypes = [ctypes.c_int32] * 4 + [c_f] * 2 + [ctypes.c_float] + [c_f] * 3
+    lib.mvp_debug_heavy_offset.restype = ctypes.c_size_t
+    lib.mvp_debug_heavy_offset.argtypes = [ctypes.POINTER(Shape)]
     lib.mvp_forward_launch_count.restype = ctypes.c_int
     lib.mvp_forward_launch_count.argtypes = [ctypes.c_uint32]
     lib.mvp_backward_launch_count.restype = ctypes.c_int

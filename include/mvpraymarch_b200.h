@@ -233,6 +233,10 @@ int mvp_sum_views(const float *src, float *dst, size_t count, int32_t n_views, v
 int mvp_debug_saved_tiles(const mvp_shape *shape, const void *host_workspace_copy, int *saved, int *not_saved);
 /* Diagnostics builds only (-DMVP_TILE_CLOCKS=1, scripts/tile_clocks.py): byte offset of the per-tile clock records in the workspace. */
 size_t mvp_debug_tileclk_offset(const mvp_shape *shape);
+/* Test / diagnostics helper (host only, no device work): byte offset in the workspace of the int32 count of "heavy" tiles, the
+ * tiles whose slab list did not fit the fast render kernel's list and that the 512-entry kernel rendered.  Every forward and
+ * backward call resets it first, so the 4 bytes read after a call are that call's count; 0 for an invalid shape. */
+size_t mvp_debug_heavy_offset(const mvp_shape *shape);
 
 /* Number of kernels the last forward / backward call of this shape launches (for bench.py's gpu_launches). */
 int mvp_forward_launch_count(uint32_t flags);

@@ -12,6 +12,7 @@ from tests.emul.build import build_kernels
 _LIBS = {}
 _variant = ()
 _opt = "-O1"
+last_heavy_tiles = (0, 0)   # (forward, backward) heavy-tile counts of the last forward_backward call (mvp_debug_heavy_offset)
 
 
 def use_variant(defines=(), opt="-O1"):
@@ -32,6 +33,8 @@ def load():
         L.mvp_raymarch_backward.restype = ctypes.c_int
         L.mvp_raymarch_backward.argtypes = [ctypes.POINTER(_abi.BackwardArgs), ctypes.c_void_p]
         L.mvp_abi_version.restype = ctypes.c_int
+        L.mvp_debug_heavy_offset.restype = ctypes.c_size_t
+        L.mvp_debug_heavy_offset.argtypes = [ctypes.POINTER(_abi.Shape)]
         assert L.mvp_abi_version() == _abi.ABI_VERSION
         _LIBS[key] = L
     return _LIBS[key]
@@ -72,7 +75,9 @@ def forward_backward(raypos, raydir, stepsize, tminmax, primpos, primrot, primsc
     clear_in_forward: the gradient buffers are handed to the forward NaN-filled (mvp_forward_args::clear_grad_*), which must leave
     them zero; the backward then runs without MVP_FLAG_ZERO_GRADS.
     camera = (viewpos, viewrot, focal, princpt, volradius, H, W): the kernels generate the rays (mvp_camera); raypos / raydir / tminmax
-    must then be None and are passed as NULL."""
+    must then be None and are passed as NULL.
+    The numbers of heavy tiles (rendered by the 512-entry kernels) of the forward and the backward are left in last_heavy_tiles."""
+    global last_heavy_tiles
     L = load()
     primpos, primrot, primscale, template = map(_f32, (primpos, primrot, primscale, template))
     warp = None if warp is None else _f32(warp)
@@ -91,6 +96,8 @@ def forward_backward(raypos, raydir, stepsize, tminmax, primpos, primrot, primsc
     wsb = L.mvp_workspace_bytes(ctypes.byref(shape))
     assert wsb > 0
     ws = _aligned(wsb)
+    hoff = L.mvp_debug_heavy_offset(ctypes.byref(shape))
+    heavy = lambda: int(ws[hoff:hoff + 4].view(np.int32)[0])  # noqa: E731
     rayrgba = np.full((N, H, W, 4), np.nan, np.float32)
     want_grad = grad_rayrgba is not None
     raysat = np.full((N, H, W, 3), np.nan, np.float32) if want_grad else None
@@ -123,6 +130,7 @@ def forward_backward(raypos, raydir, stepsize, tminmax, primpos, primrot, primsc
         a.clear_grad_warp = _p(pre[4])
     rc = L.mvp_raymarch_forward(ctypes.byref(a), None)
     assert rc == 0, rc
+    last_heavy_tiles = (heavy(), 0)
     if pre is not None:
         assert all(g is None or not g.any() for g in pre), "the forward must leave the clear_grad_* buffers zero"
     if planes:                      # hand back the same layout as the channels-last run, assembled from the planes
@@ -155,6 +163,7 @@ def forward_backward(raypos, raydir, stepsize, tminmax, primpos, primrot, primsc
         b.WD, b.WH, b.WW = warp.shape[2:5]
     rc = L.mvp_raymarch_backward(ctypes.byref(b), None)
     assert rc == 0, rc
+    last_heavy_tiles = (last_heavy_tiles[0], heavy())
     if gwarp is not None:
         grads.append(gwarp)
     return rayrgba, raysat, grads

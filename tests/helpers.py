@@ -53,6 +53,41 @@ def make_warp(N, K, WD, WH, WW, seed=77, amp=0.05):
     return (grid + amp * torch.randn(N, K, WD, WH, WW, 3, generator=g)).contiguous()
 
 
+def dense_scene(N=1, H=17, W=27, k3=7, M=4, dims=None, seed=5, warp=False, gain=(0.05, 1.0)):
+    """k3^3 large slabs that overlap on every pixel: every 8x4 tile's slab list holds all of them (k3 = 7: 343 entries, past the
+    256 of the fast render kernels; k3 >= 9: more than the reference's 512-entry cap).  K stays below the 2048-entry row bucket, so
+    the lists are built from the TMA-staged bucket, not from the row-overflow scan.  Every ray crosses every slab, so a uniform
+    alpha gain leaves either no ray or every ray saturated; here the gain is log-uniform per slab in `gain` * 343 / K and each
+    ray ends at its own depth inside the slab cloud (tmax = tmin + 2.5 ... 6.5), which saturates a part of the rays.  H and W
+    that are not multiples of 4 and 8 give partial tiles."""
+    s = gradcheck_like_scene(N=N, H=H, W=W, k3=k3, M=M, seed=seed, alpha_gain=1.0, scale=1.1, dims=dims)
+    K = k3 ** 3
+    g = torch.Generator().manual_seed(seed + 1)
+    lo, hi = (x * 343.0 / K for x in gain)
+    s["template"][..., 3] *= (lo * (hi / lo) ** torch.rand(N, K, generator=g)).view(N, K, 1, 1, 1)
+    s["tminmax"][..., 1] = s["tminmax"][..., 0] + 2.5 + 4.0 * torch.rand(N, H, W, generator=g)
+    if warp:
+        s["warp"] = make_warp(N, K, 3, 4, 5, seed=seed + 2, amp=0.05)
+    return s
+
+
+# Dense scenes whose tiles are all "heavy" (slab list > 256 entries: rendered by the 512-entry kernels), one per instantiation of
+# those kernels (T = 8, 16, runtime dims; algo 1 = runtime dims with a warp field), each without and with the 512-entry cap hit.
+DENSE_CASES = {
+    "t8": lambda k3: dense_scene(N=2, k3=k3, M=8, seed=5),
+    "t16": lambda k3: dense_scene(N=1, H=14, W=19, k3=k3, M=16, seed=6),
+    "noncubic": lambda k3: dense_scene(N=2, H=13, W=21, k3=k3, dims=(3, 5, 4), seed=7),
+    "warp": lambda k3: dense_scene(N=2, H=18, W=22, k3=k3, M=4, seed=8, warp=True),
+}
+DENSE_K3 = {"uncapped": 7, "capped": 9}
+
+
+def build_dense_case(name, cap):
+    s = DENSE_CASES[name](DENSE_K3[cap])
+    g = torch.Generator().manual_seed(4243)
+    return s, torch.randn(*s["raypos"].shape[:3], 4, generator=g)
+
+
 def scene_args_np(s, dtype=np.float32):
     """(positional args for oracle.forward, kwargs)."""
     a = [s["raypos"].numpy().astype(dtype), s["raydir"].numpy().astype(dtype), float(s["stepsize"]),
@@ -95,7 +130,8 @@ CASES = {
     "gradcheck_ragged": lambda: gradcheck_like_scene(N=1, H=13, W=19, k3=3, M=4, seed=7, alpha_gain=8.0),
     # head scene, C1-like but small: pinhole dome cameras, UV-grid slabs on an ellipsoid
     "head_small": lambda: _head_case(2, 64, 42, 64, 8, stepsize=1.0 / 64, alpha_mu=1.0, alpha_sigma=2.0),
-    # 125 large overlapping slabs: every tile sees > 96 candidates -> exercises the 512-entry kernel variant
+    # 125 large overlapping slabs: every tile sees > 96 candidates; the lists stay below the fast kernels' 256 entries (the
+    # 512-entry kernels: DENSE_CASES, tests/test_gpu_heavy_tiles.py)
     "many_overlaps": lambda: gradcheck_like_scene(N=1, H=12, W=20, k3=5, M=4, seed=3, alpha_gain=0.4, scale=1.1),
     # non-cubic payload (runtime-stride sampler path) incl. a 1-voxel axis
     "noncubic": lambda: gradcheck_like_scene(N=1, H=14, W=17, k3=2, seed=21, alpha_gain=30.0, dims=(3, 1, 5)),
