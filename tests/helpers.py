@@ -88,6 +88,97 @@ def build_dense_case(name, cap):
     return s, torch.randn(*s["raypos"].shape[:3], 4, generator=g)
 
 
+ABI_GRAD_NAMES = ("primpos", "primrot", "primscale", "template", "warp")
+
+
+def abi_raymarch(s, grad=None, fwd_flags=0, order=None, planes=False, camera=None, shared=False, keep=None, clear_in_forward=False):
+    """Forward (+ backward when `grad` is given) of scene `s` (CUDA tensors) straight through the C-ABI.  camera =
+    (viewpos, viewrot, focal, princpt, volradius, H, W): rays generated in the kernels, s's ray tensors are not passed.
+    The gradient buffers start as NaN; the backward zero-fills them (MVP_FLAG_ZERO_GRADS), or, with clear_in_forward, the
+    forward's render kernel does (clear_grad_*) and the backward runs without the flag, as the op does.
+    Returns (rayrgba, raysat, grads or None, (heavy tiles of the forward, of the backward)); when `keep` is a dict it receives
+    the workspace ("workspace") and rayaux ("rayaux")."""
+    import ctypes
+    from ava256_b200 import lib
+    P = lambda x: None if x is None else ctypes.c_void_p(x.data_ptr())  # noqa: E731
+    K = s["primpos"].shape[1]
+    if camera is not None:
+        N, H, W = camera[0].shape[0], camera[5], camera[6]
+        cam = lib.Camera(P(camera[0]), P(camera[1]), P(camera[2]), P(camera[3]), float(camera[4]), 0)
+        rays = (None, None, None)
+    else:
+        N, H, W = s["raypos"].shape[:3]
+        cam = lib.Camera()
+        rays = (s["raypos"], s["raydir"], s["tminmax"])
+    TD, TH, TW = s["template"].shape[2:5]
+    shape = lib.Shape(N, H, W, K, TD, TH, TW)
+    wsb = lib.workspace_bytes(N, H, W, K, TD, TH, TW)
+    ws = torch.empty(wsb, dtype=torch.uint8, device="cuda")
+    hoff = lib.LIB.mvp_debug_heavy_offset(ctypes.byref(shape))
+    heavy = lambda: int(ws[hoff:hoff + 4].view(torch.int32).item())  # noqa: E731
+    warp = s.get("warp")
+    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    sh = lib.FLAG_SHARED_PRIMS if shared else 0
+    rgba = torch.full((N, H, W, 4), float("nan"), device="cuda")
+    rgb_p = torch.full((N, 3, H, W), float("nan"), device="cuda") if planes else None
+    alpha_p = torch.full((N, 1, H, W), float("nan"), device="cuda") if planes else None
+    rsat = torch.empty(N, H, W, 3, device="cuda") if grad is not None else None
+    raux = torch.empty(N, H, W, 4, dtype=torch.int32, device="cuda") if grad is not None else None
+    if keep is not None:
+        keep["workspace"], keep["rayaux"] = ws, raux
+    gs = None
+    if grad is not None:
+        gs = [torch.full_like(s[n], float("nan")) for n in ABI_GRAD_NAMES[:4]] + \
+             ([torch.full_like(warp, float("nan"))] if warp is not None else [])
+    a = lib.ForwardArgs()
+    a.shape, a.stepsize, a.fadescale, a.fadeexp = shape, s["stepsize"], s.get("fadescale", 8.0), s.get("fadeexp", 8.0)
+    a.flags = fwd_flags | sh
+    a.raypos, a.raydir, a.tminmax = (P(x) for x in rays)
+    a.camera = cam
+    a.primpos, a.primrot, a.primscale, a.tplate = P(s["primpos"]), P(s["primrot"]), P(s["primscale"]), P(s["template"])
+    a.rayrgba, a.raysat, a.rayaux = (None if planes else P(rgba)), P(rsat), P(raux)
+    a.rayrgb_nchw, a.rayalpha_nchw = P(rgb_p), P(alpha_p)
+    a.order = P(order)
+    a.workspace, a.workspace_bytes = P(ws), wsb
+    if warp is not None:
+        a.algo, a.warp = 1, P(warp)
+        a.WD, a.WH, a.WW = warp.shape[2:5]
+    if clear_in_forward:
+        assert gs is not None, "the forward clears the gradient buffers of a backward"
+        a.clear_grad_primpos, a.clear_grad_primrot, a.clear_grad_primscale, a.clear_grad_tplate = (P(g) for g in gs[:4])
+        a.clear_grad_warp = P(gs[4]) if warp is not None else None
+    lib.check(lib.LIB.mvp_raymarch_forward(ctypes.byref(a), st))
+    hf = heavy()
+    if planes:
+        rgba = torch.cat([rgb_p, alpha_p], dim=1).permute(0, 2, 3, 1).contiguous()
+    if grad is None:
+        torch.cuda.synchronize()
+        return rgba, None, None, (hf, 0)
+    b = lib.BackwardArgs()
+    b.shape, b.stepsize, b.fadescale, b.fadeexp = a.shape, a.stepsize, a.fadescale, a.fadeexp
+    b.flags = lib.FLAG_ACCEL_VALID | (0 if clear_in_forward else lib.FLAG_ZERO_GRADS) | sh
+    b.raypos, b.raydir, b.tminmax = a.raypos, a.raydir, a.tminmax
+    b.camera = cam
+    b.primpos, b.primrot, b.primscale, b.tplate = a.primpos, a.primrot, a.primscale, a.tplate
+    if planes:
+        gp = grad.permute(0, 3, 1, 2)
+        g_rgb, g_alpha = gp[:, :3].contiguous(), gp[:, 3:4].contiguous()
+        b.grad_rayrgb_nchw, b.grad_rayalpha_nchw = P(g_rgb), P(g_alpha)
+    else:
+        b.grad_rayrgba = P(grad)
+    b.raysat, b.rayaux = P(rsat), P(raux)
+    b.grad_primpos, b.grad_primrot, b.grad_primscale, b.grad_tplate = (P(g) for g in gs[:4])
+    b.order = a.order
+    b.workspace, b.workspace_bytes = P(ws), wsb
+    if warp is not None:
+        b.algo, b.warp, b.grad_warp = 1, P(warp), P(gs[4])
+        b.WD, b.WH, b.WW = a.WD, a.WH, a.WW
+    lib.check(lib.LIB.mvp_raymarch_backward(ctypes.byref(b), st))
+    hb = heavy()
+    torch.cuda.synchronize()
+    return rgba, rsat, gs, (hf, hb)
+
+
 def scene_args_np(s, dtype=np.float32):
     """(positional args for oracle.forward, kwargs)."""
     a = [s["raypos"].numpy().astype(dtype), s["raydir"].numpy().astype(dtype), float(s["stepsize"]),

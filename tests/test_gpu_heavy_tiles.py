@@ -5,12 +5,10 @@ The scenes of tests/helpers.py DENSE_CASES make every tile heavy; each test read
 backward call back from the workspace (`mvp_debug_heavy_offset`) and asserts that the path ran.  Gates as in the rest of the
 suite: forward max|d|/max|ref| <= 1e-4 and gradients <= 1e-3 against the oracle; 1e-5 between runs that differ only in the
 order of the gradient atomics."""
-import ctypes
-
 import pytest
 import torch
 
-from tests.helpers import DENSE_CASES, DENSE_K3, build_dense_case, dense_scene, relerr, scene_args_np
+from tests.helpers import DENSE_CASES, DENSE_K3, abi_raymarch, build_dense_case, dense_scene, relerr, scene_args_np
 
 pytestmark = pytest.mark.gpu
 
@@ -18,84 +16,6 @@ FWD_TOL = 1e-4
 BWD_TOL = 1e-3
 NAMES = ("primpos", "primrot", "primscale", "template", "warp")
 HEAVY_CTAS_PER_SM = 4          # kHeavyCtasPerSM in csrc/mvp_kernels.cu: the persistent grid is 4 CTAs per SM
-
-
-def _abi(s, grad=None, fwd_flags=0, order=None, planes=False, camera=None, shared=False, keep_ws=None):
-    """Forward (+ backward when `grad` is given) of scene `s` (CUDA tensors) straight through the C-ABI.  camera =
-    (viewpos, viewrot, focal, princpt, volradius, H, W): rays generated in the kernels, s's ray tensors are not passed.
-    Returns (rayrgba, raysat, grads or None, (heavy tiles of the forward, of the backward)); the workspace is appended to
-    `keep_ws` when that is a list."""
-    from ava256_b200 import lib
-    P = lambda x: None if x is None else ctypes.c_void_p(x.data_ptr())  # noqa: E731
-    K = s["primpos"].shape[1]
-    if camera is not None:
-        N, H, W = camera[0].shape[0], camera[5], camera[6]
-        cam = lib.Camera(P(camera[0]), P(camera[1]), P(camera[2]), P(camera[3]), float(camera[4]), 0)
-        rays = (None, None, None)
-    else:
-        N, H, W = s["raypos"].shape[:3]
-        cam = lib.Camera()
-        rays = (s["raypos"], s["raydir"], s["tminmax"])
-    TD, TH, TW = s["template"].shape[2:5]
-    shape = lib.Shape(N, H, W, K, TD, TH, TW)
-    wsb = lib.workspace_bytes(N, H, W, K, TD, TH, TW)
-    ws = torch.empty(wsb, dtype=torch.uint8, device="cuda")
-    if keep_ws is not None:
-        keep_ws.append(ws)
-    hoff = lib.LIB.mvp_debug_heavy_offset(ctypes.byref(shape))
-    heavy = lambda: int(ws[hoff:hoff + 4].view(torch.int32).item())  # noqa: E731
-    warp = s.get("warp")
-    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    sh = lib.FLAG_SHARED_PRIMS if shared else 0
-    rgba = torch.full((N, H, W, 4), float("nan"), device="cuda")
-    rgb_p = torch.full((N, 3, H, W), float("nan"), device="cuda") if planes else None
-    alpha_p = torch.full((N, 1, H, W), float("nan"), device="cuda") if planes else None
-    rsat = torch.empty(N, H, W, 3, device="cuda") if grad is not None else None
-    raux = torch.empty(N, H, W, 4, dtype=torch.int32, device="cuda") if grad is not None else None
-    a = lib.ForwardArgs()
-    a.shape, a.stepsize, a.fadescale, a.fadeexp = shape, s["stepsize"], s.get("fadescale", 8.0), s.get("fadeexp", 8.0)
-    a.flags = fwd_flags | sh
-    a.raypos, a.raydir, a.tminmax = (P(x) for x in rays)
-    a.camera = cam
-    a.primpos, a.primrot, a.primscale, a.tplate = P(s["primpos"]), P(s["primrot"]), P(s["primscale"]), P(s["template"])
-    a.rayrgba, a.raysat, a.rayaux = (None if planes else P(rgba)), P(rsat), P(raux)
-    a.rayrgb_nchw, a.rayalpha_nchw = P(rgb_p), P(alpha_p)
-    a.order = P(order)
-    a.workspace, a.workspace_bytes = P(ws), wsb
-    if warp is not None:
-        a.algo, a.warp = 1, P(warp)
-        a.WD, a.WH, a.WW = warp.shape[2:5]
-    lib.check(lib.LIB.mvp_raymarch_forward(ctypes.byref(a), st))
-    hf = heavy()
-    if planes:
-        rgba = torch.cat([rgb_p, alpha_p], dim=1).permute(0, 2, 3, 1).contiguous()
-    if grad is None:
-        torch.cuda.synchronize()
-        return rgba, None, None, (hf, 0)
-    gs = [torch.full_like(s[n], float("nan")) for n in NAMES[:4]] + ([torch.full_like(warp, float("nan"))] if warp is not None else [])
-    b = lib.BackwardArgs()
-    b.shape, b.stepsize, b.fadescale, b.fadeexp = a.shape, a.stepsize, a.fadescale, a.fadeexp
-    b.flags = lib.FLAG_ACCEL_VALID | lib.FLAG_ZERO_GRADS | sh
-    b.raypos, b.raydir, b.tminmax = a.raypos, a.raydir, a.tminmax
-    b.camera = cam
-    b.primpos, b.primrot, b.primscale, b.tplate = a.primpos, a.primrot, a.primscale, a.tplate
-    if planes:
-        gp = grad.permute(0, 3, 1, 2)
-        g_rgb, g_alpha = gp[:, :3].contiguous(), gp[:, 3:4].contiguous()
-        b.grad_rayrgb_nchw, b.grad_rayalpha_nchw = P(g_rgb), P(g_alpha)
-    else:
-        b.grad_rayrgba = P(grad)
-    b.raysat, b.rayaux = P(rsat), P(raux)
-    b.grad_primpos, b.grad_primrot, b.grad_primscale, b.grad_tplate = (P(g) for g in gs[:4])
-    b.order = a.order
-    b.workspace, b.workspace_bytes = P(ws), wsb
-    if warp is not None:
-        b.algo, b.warp, b.grad_warp = 1, P(warp), P(gs[4])
-        b.WD, b.WH, b.WW = a.WD, a.WH, a.WW
-    lib.check(lib.LIB.mvp_raymarch_backward(ctypes.byref(b), st))
-    hb = heavy()
-    torch.cuda.synchronize()
-    return rgba, rsat, gs, (hf, hb)
 
 
 def _cuda(s):
@@ -127,13 +47,13 @@ def test_heavy_kernels_vs_oracle(name, cap):
     lists of 729 cut at the reference's 512; the inference-mode forward (kGrad = false) gives the same image bits."""
     s, grad = build_dense_case(name, cap)
     t = _cuda(s)
-    out, rsat, grads, heavy = _abi(t, grad.cuda())
+    out, rsat, grads, heavy = abi_raymarch(t, grad.cuda())
     _report("%s/%s" % (name, cap), heavy)
     sat = float((out[..., 3] >= 1.0).float().mean())
     assert 0.1 <= sat <= 0.9, sat
     stats = _vs_oracle(s, grad, out, grads)
     assert (stats["capped_warps"] > 0) == (cap == "capped"), stats
-    out_i, _, _, heavy_i = _abi(t)
+    out_i, _, _, heavy_i = abi_raymarch(t)
     assert heavy_i[0] == heavy[0]
     assert torch.equal(out_i, out)
 
@@ -153,16 +73,16 @@ def test_heavy_persistent_loop_walks_every_tile():
     s = dense_scene(N=N, H=H, W=W, k3=7, M=8, seed=9, gain=(0.02, 0.4))   # few saturated rays (see test_emul_kernels.py)
     grad = torch.randn(N, H, W, 4, generator=torch.Generator().manual_seed(7))
     t, g = _cuda(s), grad.cuda()
-    out, _, grads, heavy = _abi(t, g)
+    out, _, grads, heavy = abi_raymarch(t, g)
     _report("persistent %dx%dx%d, %d heavy-grid warps on %d SMs" % (N, H, W, grid_warps, sms), heavy)
     assert heavy[0] >= 2 * grid_warps and heavy[1] >= 2 * grid_warps, (heavy, grid_warps)
-    out2, _, grads2, heavy2 = _abi(t, g)
+    out2, _, grads2, heavy2 = abi_raymarch(t, g)
     assert heavy2 == heavy and torch.equal(out2, out)
     for x, y in zip(grads, grads2):
         assert relerr(x.cpu().numpy(), y.cpu().numpy()) <= 1e-5
     for v in range(N):
         sv = {k: (x[v:v + 1].contiguous() if torch.is_tensor(x) else x) for k, x in t.items()}
-        out_v, _, grads_v, heavy_v = _abi(sv, g[v:v + 1].contiguous())
+        out_v, _, grads_v, heavy_v = abi_raymarch(sv, g[v:v + 1].contiguous())
         assert heavy_v[0] > 0 and torch.equal(out_v, out[v:v + 1])
         for nm, x, y in zip(NAMES, grads_v, grads):
             assert relerr(x.cpu().numpy(), y[v:v + 1].cpu().numpy()) <= 1e-5, (v, nm)
@@ -180,13 +100,13 @@ def test_heavy_backward_saved_lists_equal_rebuilt(cap):
     t, g = _cuda(s), grad.cuda()
     N, H, W = s["raypos"].shape[:3]
     K, T = s["primpos"].shape[1], s["template"].shape[2]
-    ws0, ws1 = [], []
-    out0, _, g0, heavy0 = _abi(t, g, keep_ws=ws0)
+    ws0, ws1 = {}, {}
+    out0, _, g0, heavy0 = abi_raymarch(t, g, keep=ws0)
     _report("saved lists/%s" % cap, heavy0)
-    out1, _, g1, heavy1 = _abi(t, g, fwd_flags=lib.FLAG_TEST_TINY_LISTS, keep_ws=ws1)
+    out1, _, g1, heavy1 = abi_raymarch(t, g, fwd_flags=lib.FLAG_TEST_TINY_LISTS, keep=ws1)
     _report("rebuilt lists/%s" % cap, heavy1)
-    saved0, not_saved0 = _saved_tiles(ws0[0], N, H, W, K, T)
-    saved1, not_saved1 = _saved_tiles(ws1[0], N, H, W, K, T)
+    saved0, not_saved0 = _saved_tiles(ws0["workspace"], N, H, W, K, T)
+    saved1, not_saved1 = _saved_tiles(ws1["workspace"], N, H, W, K, T)
     tiles = N * -(-H // 4) * -(-W // 8)
     assert heavy0[0] == tiles and saved0 > 0, (heavy0, saved0, not_saved0)  # heavy tiles whose saved list the backward loads
     assert not_saved1 == tiles, (saved1, not_saved1)                         # every tile rebuilt
@@ -201,8 +121,8 @@ def test_heavy_shared_primitives_equal_materialised():
     grad = torch.randn(3, 17, 27, 4, device="cuda", generator=torch.Generator(device="cuda").manual_seed(2))
     one = {k: (v[:1].contiguous() if k in NAMES else v) for k, v in s.items()}
     rep = {k: (v[:1].expand_as(v).contiguous() if k in NAMES else v) for k, v in s.items()}
-    out_m, _, g_m, heavy_m = _abi(rep, grad)
-    out_s, _, g_s, heavy_s = _abi(one, grad, shared=True)
+    out_m, _, g_m, heavy_m = abi_raymarch(rep, grad)
+    out_s, _, g_s, heavy_s = abi_raymarch(one, grad, shared=True)
     _report("shared primitives", heavy_s)
     assert heavy_s == heavy_m and torch.equal(out_s, out_m)
     for nm, x, y in zip(NAMES, g_m, g_s):
@@ -219,12 +139,12 @@ def test_heavy_marching_order_equals_gathered(cap):
     t, g = _cuda(s), grad.cuda()
     order = morton_order(t["primpos"]).to(torch.int32).contiguous()
     assert not torch.equal(order, torch.arange(order.size(1), device="cuda", dtype=torch.int32).expand_as(order))
-    out_o, _, g_o, heavy_o = _abi(t, g, order=order)
+    out_o, _, g_o, heavy_o = abi_raymarch(t, g, order=order)
     _report("marching order/%s" % cap, heavy_o)
     idx = order.long()
     take = lambda x: torch.gather(x, 1, idx.view(idx.shape + (1,) * (x.dim() - 2)).expand(idx.shape + tuple(x.shape[2:]))).contiguous()  # noqa: E731
     tg = {k: (take(v) if k in NAMES else v) for k, v in t.items()}
-    out_g, _, g_g, heavy_g = _abi(tg, g)
+    out_g, _, g_g, heavy_g = abi_raymarch(tg, g)
     assert heavy_g == heavy_o and torch.equal(out_o, out_g)
     for nm, x, y in zip(NAMES, g_o, g_g):
         back = torch.zeros_like(y).scatter_(1, idx.view(idx.shape + (1,) * (y.dim() - 2)).expand_as(y), y)
@@ -237,8 +157,8 @@ def test_heavy_image_planes_equal_channels_last(name):
     prologue == the channels-last run (forward bit for bit)."""
     s, grad = build_dense_case(name, "uncapped")
     t, g = _cuda(s), grad.cuda()
-    out0, _, g0, heavy0 = _abi(t, g)
-    out1, _, g1, heavy1 = _abi(t, g, planes=True)
+    out0, _, g0, heavy0 = abi_raymarch(t, g)
+    out1, _, g1, heavy1 = abi_raymarch(t, g, planes=True)
     _report("image planes/%s" % name, heavy1)
     assert heavy1 == heavy0 and torch.equal(out0, out1)
     for nm, x, y in zip(NAMES, g0, g1):
@@ -255,8 +175,8 @@ def test_heavy_camera_rays_equal_two_call_form():
     cams = [c.cuda() for c in scene.make_cameras(n, H, W, view_offset=3)]
     rp, rd, tmm = compute_raydirs(cams[0], cams[1], cams[2], cams[3], (W, H), scene.VOLRADIUS)
     grad = torch.randn(n, H, W, 4, device="cuda", generator=torch.Generator(device="cuda").manual_seed(1))
-    out_t, _, g_t, heavy_t = _abi(dict(s, raypos=rp, raydir=rd, tminmax=tmm), grad)
-    out_c, _, g_c, heavy_c = _abi(s, grad, camera=tuple(cams) + (scene.VOLRADIUS, H, W))
+    out_t, _, g_t, heavy_t = abi_raymarch(dict(s, raypos=rp, raydir=rd, tminmax=tmm), grad)
+    out_c, _, g_c, heavy_c = abi_raymarch(s, grad, camera=tuple(cams) + (scene.VOLRADIUS, H, W))
     _report("camera rays", heavy_c)
     assert heavy_c == heavy_t
     assert float(out_t[..., 3].max()) > 0.05 and torch.equal(out_t, out_c)

@@ -93,8 +93,8 @@ def test_non_pinhole_rays_fall_back():
 
 def test_reference_extension_side_by_side():
     """Mid-size head scene against the reference kernels (their outputs stored in tests/golden/scale_head_256x168.npz)."""
-    from tests.test_gpu_scale_parity import assert_parity_with_golden
-    assert_parity_with_golden("head_256x168")
+    from tests.test_gpu_scale_parity import assert_scale_case_parity
+    assert_scale_case_parity("head_256x168")
 
 
 @pytest.mark.parametrize("kind", ["zero_scale", "rays_miss_volume", "large_step", "tiny_step"])

@@ -40,10 +40,9 @@ def _ours(s, grad):
     return out.detach(), [x.grad for x in lv]
 
 
-def assert_parity_with_golden(name):
-    """This library's fwd+bwd of tests/helpers.py scale_case(name) against the reference's stored outputs."""
-    s, grad = scale_case(name)
-    out, grads = _ours(s, grad)
+def assert_parity_with_golden(out, grads, name):
+    """This library's rayrgba `out` and gradients `grads` (primpos, primrot, primscale, template) of the inputs of
+    tests/helpers.py scale_case(name) against the reference's stored outputs."""
     gold = np.load(os.path.join(GOLDEN, "scale_%s.npz" % name))
     d, l1 = sampled_relerr(gold, "rayrgba", out)
     r = reductions_relerr(gold, "rayrgba", out)
@@ -62,9 +61,15 @@ def assert_parity_with_golden(name):
         assert d <= BWD_TOL and l1 <= BWD_TOL and r <= BWD_TOL, (nm, d, l1, r)
 
 
+def assert_scale_case_parity(name):
+    """This library's fwd+bwd of scale_case(name) against the reference's stored outputs."""
+    out, grads = _ours(*scale_case(name))
+    assert_parity_with_golden(out, grads, name)
+
+
 def test_c2_full_size_vs_reference_extension():
     """BASELINE.json config 2: 1 subject, 4 views 512x334, K=4096, 16^3, fwd+bwd vs the reference mvpraymarch."""
-    assert_parity_with_golden("c2")
+    assert_scale_case_parity("c2")
 
 
 def test_c3_bench_scene_vs_reference_extension():
@@ -73,7 +78,7 @@ def test_c3_bench_scene_vs_reference_extension():
     import bench
     assert (bench.H, bench.W, bench.K, bench.T, bench.ALPHA_MU, bench.ALPHA_SIGMA) == (1024, 667, 16384, 8, 17.0, 6.0)
     for name in ("c3_view0", "c3_view78"):
-        assert_parity_with_golden(name)
+        assert_scale_case_parity(name)
         torch.cuda.empty_cache()
 
 
