@@ -1060,6 +1060,7 @@ struct Params {
 #if defined(MVP_CPU_EMUL) && defined(MVP_EMUL_STATS)
 long long g_emul_list_chunks;   // 32-entry bucket chunks scanned by build_tile_list (forward + backward)
 long long g_emul_bwd_stats[8];  // see render_backward_kernel
+long long g_emul_bwd_groups[32], g_emul_bwd_voxels;
 #endif
 
 // No slab rectangle reaches this tile (three quarters of the tiles of a head-and-shoulders view): its rays hit nothing, whatever they
@@ -1798,11 +1799,19 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
 // ------------------------------------------------------------------------------------------------------
 // 5. backward (slab-major)
 // ------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void red_add_v4(float *addr, float a, float b, float c, float d) {
-#ifdef MVP_EXPERIMENT_NO_RED   // timing experiment only: how much of the backward is the payload-gradient scatter?
-    if (a == 12345.678f) addr[0] = b + c + d;
-    return;
+// Mask of the lanes whose key equals this lane's; every lane of the warp takes part.  The CPU emulation of the kernels has
+// no match instruction, so there the same mask is assembled from 32 shuffles.
+__device__ __forceinline__ unsigned match_any_warp(int key) {
+#ifdef MVP_CPU_EMUL
+    unsigned m = 0;
+    for (int j = 0; j < 32; ++j) m |= (__shfl_sync(0xffffffffu, key, j) == key ? 1u : 0u) << j;
+    return m;
+#else
+    return __match_any_sync(0xffffffffu, key);
 #endif
+}
+
+__device__ __forceinline__ void red_add_v4(float *addr, float a, float b, float c, float d) {
     // no "memory" clobber: the gradient buffer is never read in this kernel, loads must stay free to move
 #ifdef MVP_CPU_EMUL
     atomicAdd(addr, a); atomicAdd(addr + 1, b); atomicAdd(addr + 2, c); atomicAdd(addr + 3, d);
@@ -2060,7 +2069,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                 const int maxlen = __reduce_max_sync(0xffffffffu, len);
 #if defined(MVP_CPU_EMUL) && defined(MVP_EMUL_STATS)
                 // [0] (tile, slab) visits, [1] visits with work, [2] warp steps (sum of maxlen), [3] lane steps inside a lane's
-                // interval, [4] valid lane steps (= samples), [5] batches, [6] position-carry steps
+                // interval, [4] valid lane steps (= samples), [5] batches, [6] position-carry steps, [7] see the payload scatter
                 if (lane == 0) { std::atomic_ref<long long>(g_emul_bwd_stats[0]).fetch_add(1); if (maxlen > 0) { std::atomic_ref<long long>(g_emul_bwd_stats[1]).fetch_add(1); std::atomic_ref<long long>(g_emul_bwd_stats[2]).fetch_add(maxlen); } }
                 if (maxlen > 0 && len > 0) std::atomic_ref<long long>(g_emul_bwd_stats[3]).fetch_add(len);
 #endif
@@ -2153,8 +2162,11 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         const int meta = __float_as_int(rec.w);
                         const int owner = meta & 31;
                         const bool issat = (meta & 256) != 0;
+                        // Without a warp field, lanes past the end of a short batch stay until the payload-gradient merge below
+                        // (warp-wide collectives).  They carry lane 0's sample, so every address they form is valid; they
+                        // scatter nothing and leave before the transform-gradient sums.
+                        if (kWarp && !act) continue;
                         // per-ray data of the owner lane
-                        if (!act) continue;
                         const float *pr_ = sray + owner;
                         const float oLx = pr_[0 * 32], oLy = pr_[1 * 32], oLz = pr_[2 * 32], oLw = pr_[3 * 32];
                         const float osr = pr_[4 * 32], osg = pr_[5 * 32], osb = pr_[6 * 32], osa = pr_[7 * 32], oab = pr_[8 * 32];
@@ -2215,13 +2227,52 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         gy1 = cf * pw1 * (y1 > 0.f ? 1.f : -1.f);
                         gy2 = cf * pw2 * (y2 > 0.f ? 1.f : -1.f);
                         // ---- utils.h:504-643: scatter w_c * dL_sample (zero-weight corners add 0) ----
+                        // Samples of a batch in the same voxel cell update the same 8 addresses, and L2 serialises such
+                        // reductions.  So the lanes of one cell are summed first, by pointer jumping within the group (at stage
+                        // s every lane adds the partial sum of the member 2^s places after it, then takes over that member's
+                        // successor), and only the group's lowest lane, which then holds the total, issues the 8 reductions.
+                        const unsigned grp = match_any_warp(act ? base : -1);
+                        const bool lead = act && (grp & ((1u << lane) - 1u)) == 0u;
+                        const int nxt = __ffs(grp & ~((2u << lane) - 1u)) - 1;          // next lane of the group, -1: none
+                        const int nst = 32 - __clz(__reduce_max_sync(0xffffffffu, act ? __popc(grp) : 1) - 1);   // ceil(log2(largest group))
                         float *gc = gslab + (size_t)base * 4;
 #pragma unroll
                         for (int cn = 0; cn < 8; ++cn) {
                             const int o = ((cn & 1) ? sx : 0) + ((cn & 2) ? sy : 0) + ((cn & 4) ? sz : 0);
                             const float w_ = (wx_[cn & 1] * wy_[(cn >> 1) & 1]) * wz_[(cn >> 2) & 1];   // same product as above
-                            red_add_v4(gc + (size_t)o * 4, w_ * d0, w_ * d1, w_ * d2, w_ * B);
+                            float ua = w_ * d0, ub = w_ * d1, uc = w_ * d2, ud = w_ * B;
+                            for (int s = 0, nx = nxt; s < nst; ++s) {
+                                const int src = nx >= 0 ? nx : lane;
+                                const float va = __shfl_sync(0xffffffffu, ua, src), vb = __shfl_sync(0xffffffffu, ub, src);
+                                const float vc = __shfl_sync(0xffffffffu, uc, src), vd = __shfl_sync(0xffffffffu, ud, src);
+                                if (nx >= 0) { ua += va; ub += vb; uc += vc; ud += vd; }
+                                nx = __shfl_sync(0xffffffffu, nx, src);
+                            }
+                            if (lead) red_add_v4(gc + (size_t)o * 4, ua, ub, uc, ud);
                         }
+#if defined(MVP_CPU_EMUL) && defined(MVP_EMUL_STATS)
+                        // [7] payload-gradient reductions issued; g_emul_bwd_groups[g - 1]: cell groups of g samples;
+                        // g_emul_bwd_voxels: distinct voxels a batch updates (what merging across cells as well would issue / 8)
+                        if (lead) {
+                            std::atomic_ref<long long>(g_emul_bwd_stats[7]).fetch_add(8);
+                            std::atomic_ref<long long>(g_emul_bwd_groups[__popc(grp) - 1]).fetch_add(1);
+                        }
+                        {
+                            static thread_local int s_vox[kWarps][256];
+                            int *vx = s_vox[threadIdx.x >> 5];
+                            for (int cn = 0; cn < 8; ++cn)
+                                vx[cn * 32 + lane] = act ? base + ((cn & 1) ? sx : 0) + ((cn & 2) ? sy : 0) + ((cn & 4) ? sz : 0) : -1;
+                            __syncwarp();
+                            if (lane == 0) {
+                                std::vector<int> u(vx, vx + 256);
+                                std::sort(u.begin(), u.end());
+                                const long long nd = std::unique(u.begin(), u.end()) - u.begin() - (u[0] < 0 ? 1 : 0);
+                                std::atomic_ref<long long>(g_emul_bwd_voxels).fetch_add(nd);
+                            }
+                            __syncwarp();
+                        }
+#endif
+                        if (!act) continue;
                         // dL/d(index): d(weight)/d(index) is +1 on the upper corner, -1 on the lower one; on a clamped axis
                         // the reference sees the upper voxel as ITS lower corner (sign -1) and no other corner.
                         float gix = A * gp[0] + B * ga[0], giy = A * gp[1] + B * ga[1], giz = A * gp[2] + B * ga[2];
@@ -2905,6 +2956,11 @@ void mvp_emul_fwd_stats2(long long *out) {
 }
 void mvp_emul_bwd_stats(long long *out) {
     for (int i = 0; i < 8; ++i) { out[i] = g_emul_bwd_stats[i]; g_emul_bwd_stats[i] = 0; }
+}
+// out[0..31]: cell groups of 1..32 samples; out[32]: distinct voxels updated, summed over batches
+void mvp_emul_bwd_groups(long long *out) {
+    for (int i = 0; i < 32; ++i) { out[i] = g_emul_bwd_groups[i]; g_emul_bwd_groups[i] = 0; }
+    out[32] = g_emul_bwd_voxels; g_emul_bwd_voxels = 0;
 }
 long long mvp_emul_list_chunks(void) { const long long v = g_emul_list_chunks; g_emul_list_chunks = 0; return v; }
 #endif

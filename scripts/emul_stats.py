@@ -38,7 +38,15 @@ for tag, defs in VARIANTS:
     print("          forward loop: " + "  ".join("%s=%d" % (n, v) for n, v in zip(("sweep_steps", "skipped_steps", "events_same_slab_as_previous", "words_with_2plus_slabs", "events_in_such_words", "tiles_list_gt128", "tiles_list_gt160", "tiles_list_gt192"), s2)))
     bs = (ctypes.c_longlong * 8)()
     L.mvp_emul_bwd_stats(bs)
-    print("          backward: " + "  ".join("%s=%d" % (n, v) for n, v in zip(("slab_visits", "visits_with_work", "warp_steps", "lane_steps", "samples", "batches", "carry_steps"), bs)))
+    print("          backward: " + "  ".join("%s=%d" % (n, v) for n, v in zip(("slab_visits", "visits_with_work", "warp_steps", "lane_steps", "samples", "batches", "carry_steps", "payload_reds"), bs)))
+    # payload-gradient reductions: one per corner of every sample without the per-cell merge, one per corner of every cell
+    # group of a batch with it, and one per distinct voxel of a batch if corners shared between neighbouring cells were merged too
+    gr = (ctypes.c_longlong * 33)()
+    L.mvp_emul_bwd_groups(gr)
+    print("          payload reductions: unmerged=%d  per cell=%d (x%.2f fewer)  per voxel=%d (x%.2f fewer)" % (
+        8 * bs[4], bs[7], 8 * bs[4] / max(bs[7], 1), gr[32], 8 * bs[4] / max(gr[32], 1)))
+    print("          cell group sizes (groups / samples): " + "  ".join(
+        "%d:%d/%d" % (g + 1, gr[g], (g + 1) * gr[g]) for g in range(32) if gr[g]))
     if ref is None:
         ref = out
     else:
