@@ -1016,7 +1016,7 @@ struct Params {
     const RowEntry *rowlist;
     int R, rowcap;
     int TXn, TYn;
-    unsigned slab_bytes;          // TD*TH*TW*16
+    unsigned slab_bytes;          // TD*TH*TW * bytes per voxel (16 fp32, 8 bf16)
     const int *order, *rankof;    // explicit marching order (per view [K]) and its inverse, or NULL: the fixed-order rotation
     long long *tileclk;           // MVP_TILE_CLOCKS diagnostics
     int CXn, CYn;                 // CTAs (kBlkTX x kBlkTY tiles) per view in x / y
@@ -1317,13 +1317,87 @@ __device__ __forceinline__ int load_saved_tile_list(const Params &p, float rdt, 
 }
 #endif
 
+__device__ __forceinline__ void red_add_v4(float *addr, float a, float b, float c, float d) {
+    // no "memory" clobber: the gradient buffer is never read in this kernel, loads must stay free to move
+#ifdef MVP_CPU_EMUL
+    atomicAdd(addr, a); atomicAdd(addr + 1, b); atomicAdd(addr + 2, c); atomicAdd(addr + 3, d);
+#else
+    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d));
+#endif
+}
+
+// ---- voxel payload: the 4 channels (rgb, alpha) of one template voxel, fp32 (float4) or bf16 (Bf16x4, MVP_FLAG_TPLATE_BF16) ----
+// The render kernels take the payload type as a template parameter and touch the template and its gradient only through this
+// trait: load a voxel as float4, add a 4-channel gradient with one vector reduction, the size of a voxel.  All arithmetic is
+// fp32 either way: widening bf16 to fp32 is exact, so a bf16 template renders exactly like its fp32 widening, and a bf16
+// gradient is rounded once per reduction (red.global.add.noftz.v2.bf16x2: four channels in one REDG, round to nearest even).
+struct __align__(8) Bf16x4 { unsigned lo, hi; };   // channels 0 | 1 << 16 and 2 | 3 << 16 (little endian: channel 0 first)
+
+#ifdef MVP_CPU_EMUL
+// The CPU emulation of the kernels (tests/emul/) has neither instruction: fp32 -> bf16 rounded to nearest even with subnormals
+// kept and NaN kept NaN, and the bf16x2 reduction as a compare-and-swap loop.  Each half becomes bf16(old + v), the exact sum
+// rounded once: the sum of two bf16 values is exact in double, and rounding it to fp32 first cannot move it across a bf16
+// rounding boundary (8 significant bits per operand).
+inline unsigned emul_f32_to_bf16_rn(float x) {
+    const unsigned u = __float_as_uint(x);
+    if ((u & 0x7fffffffu) > 0x7f800000u) return (u >> 16) | 0x40u;
+    return (u + 0x7fffu + ((u >> 16) & 1u)) >> 16;
+}
+inline float emul_bf16_to_f32(unsigned h) { return __uint_as_float((h & 0xffffu) << 16); }
+inline void emul_red_add_bf16x2(unsigned *p, unsigned v) {
+    std::atomic_ref<unsigned> a(*p);
+    unsigned old = a.load(std::memory_order_relaxed), nw;
+    do {
+        const unsigned lo = emul_f32_to_bf16_rn((float)((double)emul_bf16_to_f32(old) + (double)emul_bf16_to_f32(v)));
+        const unsigned hi = emul_f32_to_bf16_rn((float)((double)emul_bf16_to_f32(old >> 16) + (double)emul_bf16_to_f32(v >> 16)));
+        nw = (hi << 16) | lo;
+    } while (!a.compare_exchange_weak(old, nw, std::memory_order_relaxed));
+}
+#endif
+
+// cvt.rn.bf16x2.f32 d, a, b: a -> the UPPER half of d, b -> the lower half, each rounded to nearest even
+__device__ __forceinline__ unsigned cvt_bf16x2(float a, float b) {
+#ifdef MVP_CPU_EMUL
+    return (emul_f32_to_bf16_rn(a) << 16) | emul_f32_to_bf16_rn(b);
+#else
+    unsigned d;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(a), "f"(b));
+    return d;
+#endif
+}
+
+template <typename V> struct Payload;
+// The gradient is addressed as 4-byte words (kWords per voxel): red(g, i, ...) adds to voxel i of the words at g.
+template <> struct Payload<float4> {
+    static constexpr unsigned kBytes = 16, kWords = 4;
+    static __device__ __forceinline__ float4 load(const float4 *v) { return __ldg(v); }
+    static __device__ __forceinline__ void red(float *g, size_t i, float a, float b, float c, float d) { red_add_v4(g + i * 4, a, b, c, d); }
+};
+template <> struct Payload<Bf16x4> {
+    static constexpr unsigned kBytes = 8, kWords = 2;
+    static __device__ __forceinline__ float4 load(const Bf16x4 *v) {
+        const uint2 u = __ldg(reinterpret_cast<const uint2 *>(v));   // one 64-bit read-only load (LDG.E.64.CONSTANT)
+        return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xffff0000u), __uint_as_float(u.y << 16),
+                           __uint_as_float(u.y & 0xffff0000u));
+    }
+    static __device__ __forceinline__ void red(float *g, size_t i, float a, float b, float c, float d) {
+        unsigned *const w = reinterpret_cast<unsigned *>(g + i * 2);
+        const unsigned lo = cvt_bf16x2(b, a), hi = cvt_bf16x2(d, c);   // channel a in the low half of the first word
+#ifdef MVP_CPU_EMUL
+        emul_red_add_bf16x2(w, lo); emul_red_add_bf16x2(w + 1, hi);
+#else
+        asm volatile("red.global.add.noftz.v2.bf16x2 [%0], {%1, %2};" ::"l"(w), "r"(lo), "r"(hi));
+#endif
+    }
+};
+
 // primsampler.h:44-66 + utils.h:408-502.  T > 0: cubic slab with compile-time strides; T == 0: runtime dims.
 // Only called for valid samples (|y| < 1), for which (a) the reference's +-100 clamp is a no-op and (b) the only
 // corner that can fall outside the slab is ix+1 == TW when fx rounds to exactly TW-1, with weight exactly 0.  The
 // cell is clamped to TW-2 instead and the fractions are taken against the clamped cell: identical products in all
 // other cases (fx - ix and (ix+1) - fx are the reference's expressions), weights (1, 0) in the edge case.
-template <int T>
-__device__ __forceinline__ float4 sample_slab(const float4 *__restrict__ slab, float y0, float y1, float y2, int TD, int TH, int TW,
+template <int T, typename V>
+__device__ __forceinline__ float4 sample_slab(const V *__restrict__ slab, float y0, float y1, float y2, int TD, int TH, int TW,
                                               float fadescale, float fadeexp) {
     const int td = T > 0 ? T : TD, th = T > 0 ? T : TH, tw = T > 0 ? T : TW;
     const float fade = __expf(-fadescale * (__powf(fabsf(y0), fadeexp) + __powf(fabsf(y1), fadeexp) + __powf(fabsf(y2), fadeexp)));
@@ -1339,9 +1413,10 @@ __device__ __forceinline__ float4 sample_slab(const float4 *__restrict__ slab, f
     const float bz0 = fz - (float)cz, bz1 = (float)(cz + 1) - fz;
     const int sx = tw > 1 ? 1 : 0, sy = th > 1 ? tw : 0, sz = td > 1 ? th * tw : 0;
     const int base = (cz * th + cy) * tw + cx;
-    const float4 *pc = slab + base;
-    const float4 v000 = __ldg(pc), v001 = __ldg(pc + sx), v010 = __ldg(pc + sy), v011 = __ldg(pc + sy + sx);
-    const float4 v100 = __ldg(pc + sz), v101 = __ldg(pc + sz + sx), v110 = __ldg(pc + sz + sy), v111 = __ldg(pc + sz + sy + sx);
+    const V *pc = slab + base;
+    using P = Payload<V>;
+    const float4 v000 = P::load(pc), v001 = P::load(pc + sx), v010 = P::load(pc + sy), v011 = P::load(pc + sy + sx);
+    const float4 v100 = P::load(pc + sz), v101 = P::load(pc + sz + sx), v110 = P::load(pc + sz + sy), v111 = P::load(pc + sz + sy + sx);
     // (wx * wy) * wz, left-associated like the reference; corner order tnw,tne,tsw,tse,bnw,bne,bsw,bse
     const float w00 = bx1 * by1, w01 = bx0 * by1, w10 = bx1 * by0, w11 = bx0 * by0;
     float4 acc;
@@ -1386,7 +1461,8 @@ __device__ __forceinline__ CellG cell_generic(float a0, float a1, float a2, int 
 }
 
 // primsampler.h:44-66 with dowarp = true: fade from y, warp field sampled at y, payload sampled at the warped position
-__device__ __forceinline__ float4 sample_slab_warped(const float4 *__restrict__ slab, const float *__restrict__ wk, float y0, float y1,
+template <typename V>
+__device__ __forceinline__ float4 sample_slab_warped(const V *__restrict__ slab, const float *__restrict__ wk, float y0, float y1,
                                                      float y2, const Params &p) {
     const float fade = __expf(-p.fadescale * (__powf(fabsf(y0), p.fadeexp) + __powf(fabsf(y1), p.fadeexp) + __powf(fabsf(y2), p.fadeexp)));
     const CellG cw = cell_generic(y0, y1, y2, p.WD, p.WH, p.WW);
@@ -1403,7 +1479,7 @@ __device__ __forceinline__ float4 sample_slab_warped(const float4 *__restrict__ 
 #pragma unroll
     for (int cn = 0; cn < 8; ++cn) {
         if (ct.idx[cn] >= 0) {
-            const float4 v = __ldg(slab + ct.idx[cn]);
+            const float4 v = Payload<V>::load(slab + ct.idx[cn]);
             acc.x = __fmaf_rn(ct.w[cn], v.x, acc.x); acc.y = __fmaf_rn(ct.w[cn], v.y, acc.y);
             acc.z = __fmaf_rn(ct.w[cn], v.z, acc.z); acc.w = __fmaf_rn(ct.w[cn], v.w, acc.w);
         }
@@ -1450,7 +1526,7 @@ struct __align__(16) FwdWarpSmem {   // per-warp shared state of the forward ker
 //    fits (almost all) with a small shared-memory footprint (more L1 for the voxel gathers) and flags the rest;
 //    the CAP == 512 variant then renders only the flagged tiles.
 // ------------------------------------------------------------------------------------------------------
-template <int T, bool kGrad, int CAP, bool kWarp>
+template <int T, bool kGrad, int CAP, bool kWarp, typename V>
 __device__ __forceinline__ bool forward_tile(const Params &p, const int n, const int tx, const int ty, const int lane, FwdWarpSmem<CAP, kGrad> *const S) {
     // all per-warp shared state lives in one record: every address below is (one pinned per-warp base) + immediate
     int *const sk = S->k, *const siv = S->iv, *const rm = S->rm;
@@ -1521,7 +1597,7 @@ __device__ __forceinline__ bool forward_tile(const Params &p, const int n, const
     // voxels per slab: a compile-time constant for the cubic 8^3 / 16^3 specialisations, so that a slab's address is a shift and an add
     // wherever the register cap makes the compiler re-derive it (it was ~30 of the 159 instructions of a batch gather)
     const size_t slabsz = T > 0 ? (size_t)(T * T * T) : (size_t)p.TD * p.TH * p.TW;
-    const float4 *tpn = reinterpret_cast<const float4 *>(p.tplate) + (size_t)(n * p.pview) * p.K * slabsz;
+    const V *tpn = reinterpret_cast<const V *>(p.tplate) + (size_t)(n * p.pview) * p.K * slabsz;
     const int kstart = dfs_kstart(p.K);
     {
         // pinned: under the register cap the compiler would otherwise re-materialise this base address per event
@@ -1576,7 +1652,7 @@ __device__ __forceinline__ bool forward_tile(const Params &p, const int n, const
         if (act) {
             const int kk = sk[(__float_as_int(rec.w) >> 5) & 1023];
             if (kWarp) sres = sample_slab_warped(tpn + (size_t)kk * slabsz, p.warp + ((size_t)(n * p.pview) * p.K + kk) * ((size_t)p.WD * p.WH * p.WW * 3), rec.x, rec.y, rec.z, p);
-            else sres = sample_slab<T>(tpn + (size_t)kk * slabsz, rec.x, rec.y, rec.z, p.TD, p.TH, p.TW, p.fadescale, p.fadeexp);
+            else sres = sample_slab<T, V>(tpn + (size_t)kk * slabsz, rec.x, rec.y, rec.z, p.TD, p.TH, p.TW, p.fadescale, p.fadeexp);
         }
         __syncwarp();
         if (act) { ring[qhead + lane] = make_float4(sres.x, sres.y, sres.z, rec.w); ra[qhead + lane] = sres.w; }
@@ -1751,7 +1827,7 @@ __device__ __forceinline__ void clear_grad_slices(const Params &p, size_t g, int
     }
 }
 
-template <int T, bool kGrad, int CAP, bool kWarp>
+template <int T, bool kGrad, int CAP, bool kWarp, typename V>
 __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_FWD_MINB * 4) / kWarps : 16 / kWarps) render_forward_kernel(const Params p) {
     __shared__ FwdWarpSmem<CAP, kGrad> s_w[kWarps];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -1762,7 +1838,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         for (int i = blockIdx.x * kWarps + warp; i < cnt; i += gridDim.x * kWarps) {
             const int id = p.heavylist[i];
             const int tx = id % p.TXn, ty = (id / p.TXn) % p.TYn, n = id / (p.TXn * p.TYn);
-            forward_tile<T, kGrad, CAP, kWarp>(p, n, tx, ty, lane, S);
+            forward_tile<T, kGrad, CAP, kWarp, V>(p, n, tx, ty, lane, S);
             __syncwarp();
         }
     } else {
@@ -1781,7 +1857,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         long long g0_;
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g0_));
 #endif
-        if (!forward_tile<T, kGrad, CAP, kWarp>(p, n, tx, ty, lane, S) && lane == 0)
+        if (!forward_tile<T, kGrad, CAP, kWarp, V>(p, n, tx, ty, lane, S) && lane == 0)
             p.heavylist[atomicAdd(p.heavycnt, 1)] = (n * p.TYn + ty) * p.TXn + tx;
 #if MVP_TILE_CLOCKS
         if (lane == 0) {
@@ -1811,26 +1887,18 @@ __device__ __forceinline__ unsigned match_any_warp(int key) {
 #endif
 }
 
-__device__ __forceinline__ void red_add_v4(float *addr, float a, float b, float c, float d) {
-    // no "memory" clobber: the gradient buffer is never read in this kernel, loads must stay free to move
-#ifdef MVP_CPU_EMUL
-    atomicAdd(addr, a); atomicAdd(addr + 1, b); atomicAdd(addr + 2, c); atomicAdd(addr + 3, d);
-#else
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d));
-#endif
-}
-
 // dL/d(index) of one sample (utils.h:591-642) in full generality, i.e. including an axis whose cell was clamped (the sample sits
 // exactly on the slab's far face: probability ~2^-24 per axis, the upper voxel is then the reference's LOWER corner and the only
 // one it sees).  Taken by those samples only; it runs after the main corner pass, when few values of the batch adjoint are live, so its
 // 12 accumulators do not add to the register peak.
-__device__ __forceinline__ float3 index_grad_general(const float4 *pc, int sx, int sy, int sz, float bx0, float bx1, float by0, float by1,
+template <typename V>
+__device__ __forceinline__ float3 index_grad_general(const V *pc, int sx, int sy, int sz, float bx0, float bx1, float by0, float by1,
                                                   float bz0, float bz1, float oLx, float oLy, float oLz, float A, float B, int clamp_mask) {
     const float wx_[2] = {bx1, bx0}, wy_[2] = {by1, by0}, wz_[2] = {bz1, bz0};
     float gpU[3] = {0.f, 0.f, 0.f}, gpL[3] = {0.f, 0.f, 0.f}, gaU[3] = {0.f, 0.f, 0.f}, gaL[3] = {0.f, 0.f, 0.f};
     for (int cn = 0; cn < 8; ++cn) {
         const int bx = cn & 1, byy = (cn >> 1) & 1, bz = (cn >> 2) & 1;
-        const float4 v = __ldg(pc + ((bx ? sx : 0) + (byy ? sy : 0) + (bz ? sz : 0)));
+        const float4 v = Payload<V>::load(pc + ((bx ? sx : 0) + (byy ? sy : 0) + (bz ? sz : 0)));
         const float pr = v.x * oLx + v.y * oLy + v.z * oLz;
         const float wyz = wy_[byy] * wz_[bz], wxz = wx_[bx] * wz_[bz], wxy = wx_[bx] * wy_[byy];
         if (bx) { gpU[0] += pr * wyz; gaU[0] += v.w * wyz; } else { gpL[0] += pr * wyz; gaL[0] += v.w * wyz; }
@@ -1886,7 +1954,7 @@ __device__ __forceinline__ Prim load_rec_shared(const float4 *rec) {
     return q;
 }
 
-template <int T, int CAP, bool kWarp>
+template <int T, int CAP, bool kWarp, typename V>
 __device__ __forceinline__ bool backward_tile(const Params &p, const int n, const int tx, const int ty, const int lane, BwdWarpSmem<CAP> *const S) {
     int *const sk = S->k, *const siv = S->iv;
     RowEntry *const sstage = S->stage;
@@ -2074,8 +2142,8 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                 if (maxlen > 0 && len > 0) std::atomic_ref<long long>(g_emul_bwd_stats[3]).fetch_add(len);
 #endif
                 if (maxlen <= 0) continue;
-                const float4 *slab = reinterpret_cast<const float4 *>(p.tplate) + (pvK + k) * slabsz;
-                float *gslab = p.g_tplate + (pvK + k) * slabsz * 4;
+                const V *slab = reinterpret_cast<const V *>(p.tplate) + (pvK + k) * slabsz;
+                float *gslab = p.g_tplate + (pvK + k) * slabsz * Payload<V>::kWords;   // as 4-byte words, see Payload
                 // transform-gradient accumulators of THIS lane for this slab: Gx[i][j] = sum xm_i * dL/dy_j and
                 // Gy[j] = sum dL/dy_j; grad_rot/scale/pos are linear in them (derived once per slab, before the reduction)
 #if MVP_BWD_LANESMEM
@@ -2194,7 +2262,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         const float bz0 = fz - (float)cz, bz1 = (float)(cz + 1) - fz;
                         const bool ex = ix > cx, ey = iy > cy, ez = iz > cz;
                         const int base = (cz * th + cy) * tw + cx;
-                        const float4 *pc = slab + base;
+                        const V *pc = slab + base;
                         // One pass over the 8 corners.  dL/d(sample) = (A dL.rgb, B) with A, B known only after the sample
                         // is complete, but <T_c, dL/d(sample)> = A <T_c.rgb, dL.rgb> + B T_c.a is linear in (A, B):
                         // accumulate the index-gradient sums for both parts now and combine afterwards.
@@ -2204,7 +2272,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
 #pragma unroll
                         for (int cn = 0; cn < 8; ++cn) {
                             const int bx = cn & 1, byy = (cn >> 1) & 1, bz = (cn >> 2) & 1;
-                            const float4 v = __ldg(pc + ((bx ? sx : 0) + (byy ? sy : 0) + (bz ? sz : 0)));
+                            const float4 v = Payload<V>::load(pc + ((bx ? sx : 0) + (byy ? sy : 0) + (bz ? sz : 0)));
                             const float w_ = (wx_[bx] * wy_[byy]) * wz_[bz];
                             sv.x = __fmaf_rn(w_, v.x, sv.x); sv.y = __fmaf_rn(w_, v.y, sv.y);
                             sv.z = __fmaf_rn(w_, v.z, sv.z); sv.w = __fmaf_rn(w_, v.w, sv.w);
@@ -2235,7 +2303,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         const bool lead = act && (grp & ((1u << lane) - 1u)) == 0u;
                         const int nxt = __ffs(grp & ~((2u << lane) - 1u)) - 1;          // next lane of the group, -1: none
                         const int nst = 32 - __clz(__reduce_max_sync(0xffffffffu, act ? __popc(grp) : 1) - 1);   // ceil(log2(largest group))
-                        float *gc = gslab + (size_t)base * 4;
+                        float *gc = gslab + (size_t)base * Payload<V>::kWords;
 #pragma unroll
                         for (int cn = 0; cn < 8; ++cn) {
                             const int o = ((cn & 1) ? sx : 0) + ((cn & 2) ? sy : 0) + ((cn & 4) ? sz : 0);
@@ -2248,7 +2316,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                                 if (nx >= 0) { ua += va; ub += vb; uc += vc; ud += vd; }
                                 nx = __shfl_sync(0xffffffffu, nx, src);
                             }
-                            if (lead) red_add_v4(gc + (size_t)o * 4, ua, ub, uc, ud);
+                            if (lead) Payload<V>::red(gc, (size_t)o, ua, ub, uc, ud);
                         }
 #if defined(MVP_CPU_EMUL) && defined(MVP_EMUL_STATS)
                         // [7] payload-gradient reductions issued; g_emul_bwd_groups[g - 1]: cell groups of g samples;
@@ -2305,7 +2373,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
 #pragma unroll
                         for (int cn = 0; cn < 8; ++cn) {
                             if (ct.idx[cn] >= 0) {
-                                const float4 v = __ldg(slab + ct.idx[cn]);
+                                const float4 v = Payload<V>::load(slab + ct.idx[cn]);
                                 sv.x = __fmaf_rn(ct.w[cn], v.x, sv.x); sv.y = __fmaf_rn(ct.w[cn], v.y, sv.y);
                                 sv.z = __fmaf_rn(ct.w[cn], v.z, sv.z); sv.w = __fmaf_rn(ct.w[cn], v.w, sv.w);
                                 const float pr = v.x * oLx + v.y * oLy + v.z * oLz;
@@ -2327,7 +2395,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         gy2 = cf * pw2 * (y2 > 0.f ? 1.f : -1.f);
 #pragma unroll
                         for (int cn = 0; cn < 8; ++cn)
-                            if (ct.idx[cn] >= 0) red_add_v4(gslab + (size_t)ct.idx[cn] * 4, ct.w[cn] * d0, ct.w[cn] * d1, ct.w[cn] * d2, ct.w[cn] * B);
+                            if (ct.idx[cn] >= 0) Payload<V>::red(gslab, (size_t)ct.idx[cn], ct.w[cn] * d0, ct.w[cn] * d1, ct.w[cn] * d2, ct.w[cn] * B);
                         // dL/d(warped position)  (utils.h:591-642), then through the warp field (primsampler.h:82-88)
                         const float e0 = gmx * (A * gp0 + B * ga0), e1_ = gmy * (A * gp1 + B * ga1), e2 = gmz * (A * gp2 + B * ga2);
                         float h0 = 0.f, h1 = 0.f, h2 = 0.f;
@@ -2426,7 +2494,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
     return true;
 }
 
-template <int T, int CAP, bool kWarp>
+template <int T, int CAP, bool kWarp, typename V>
 __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_BWD_MINB * 4) / kWarps : 12 / kWarps) render_backward_kernel(const Params p) {
     __shared__ BwdWarpSmem<CAP> s_w[kWarps];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -2436,7 +2504,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         for (int i = blockIdx.x * kWarps + warp; i < cnt; i += gridDim.x * kWarps) {
             const int id = p.heavylist[i];
             const int tx = id % p.TXn, ty = (id / p.TXn) % p.TYn, n = id / (p.TXn * p.TYn);
-            backward_tile<T, CAP, kWarp>(p, n, tx, ty, lane, S);
+            backward_tile<T, CAP, kWarp, V>(p, n, tx, ty, lane, S);
             __syncwarp();
         }
     } else {
@@ -2449,7 +2517,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         const int tx = blockIdx.x * kBlkTX + (warp % kBlkTX), ty = blockIdx.y * kBlkTY + (warp / kBlkTX), n = blockIdx.z;
 #endif
         if (tx >= p.TXn || ty >= p.TYn) return;
-        if (!backward_tile<T, CAP, kWarp>(p, n, tx, ty, lane, S) && lane == 0)
+        if (!backward_tile<T, CAP, kWarp, V>(p, n, tx, ty, lane, S) && lane == 0)
             p.heavylist[atomicAdd(p.heavycnt, 1)] = (n * p.TYn + ty) * p.TXn + tx;
     }
 }
@@ -2624,7 +2692,8 @@ int launch_accel(const mvp_shape &s, int pview, const int *order, const float *r
     return e == cudaSuccess ? MVP_OK : (int)e;
 }
 
-void fill_params(Params &p, const mvp_shape &s, float stepsize, float fadescale, float fadeexp, char *ws, const Layout &L) {
+void fill_params(Params &p, const mvp_shape &s, float stepsize, float fadescale, float fadeexp, char *ws, const Layout &L,
+                 unsigned voxel_bytes) {
     p.N = s.N; p.H = s.H; p.W = s.W; p.K = s.K; p.TD = s.TD; p.TH = s.TH; p.TW = s.TW;
     p.dt = stepsize;
     p.fadescale = fadescale; p.fadeexp = fadeexp;
@@ -2642,7 +2711,7 @@ void fill_params(Params &p, const mvp_shape &s, float stepsize, float fadescale,
     p.ctaorder = reinterpret_cast<const int *>(ws + L.ctaorder);
     p.heavycnt = reinterpret_cast<int *>(ws + L.heavycnt);
     p.heavylist = reinterpret_cast<int *>(ws + L.heavylist);
-    p.slab_bytes = (unsigned)((size_t)s.TD * s.TH * s.TW * 16);
+    p.slab_bytes = (unsigned)((size_t)s.TD * s.TH * s.TW * voxel_bytes);
 #if MVP_XBUCKETS
     p.grphdr = reinterpret_cast<const int2 *>(ws + L.grphdr);
     p.grplist = reinterpret_cast<const RowEntry *>(ws + L.grplist);
@@ -2670,7 +2739,7 @@ const char *mvp_build_config(void) {
     return "LIST_REUSE=" MVP_STR(MVP_LIST_REUSE)
            " LIST_MARGIN=" MVP_STR(MVP_LIST_MARGIN) " XBUCKETS=" MVP_STR(MVP_XBUCKETS) " FASTCAP=" MVP_STR(MVP_FWD_FASTCAP) "/" MVP_STR(MVP_BWD_FASTCAP) " SMEM_UNION=" MVP_STR(MVP_SMEM_UNION) " CARVEOUT=" MVP_STR(MVP_FWD_CARVEOUT) "/" MVP_STR(MVP_BWD_CARVEOUT) " FWD_RING=" MVP_STR(MVP_FWD_RING) " BWD_SMEMREC=" MVP_STR(MVP_BWD_SMEMREC) " BWD_LANESMEM=" MVP_STR(MVP_BWD_LANESMEM) " CTA_ORDER=" MVP_STR(MVP_CTA_ORDER) " CTA_ORDER_MIN=" MVP_STR(MVP_CTA_ORDER_MIN)
            " CHUNK=" MVP_STR(MVP_CHUNK) " FWD_MINB=" MVP_STR(MVP_FWD_MINB) " BWD_MINB=" MVP_STR(MVP_BWD_MINB)
-           " WARPS=" MVP_STR(MVP_WARPS) " BLK_TX=" MVP_STR(MVP_BLK_TX)
+           " WARPS=" MVP_STR(MVP_WARPS) " BLK_TX=" MVP_STR(MVP_BLK_TX) " TPLATE_BF16=1"
 #ifdef MVP_CPU_EMUL
            " CPU_EMUL"
 #endif
@@ -2685,7 +2754,7 @@ const char *mvp_error_string(int code) {
         case MVP_ERR_STEPSIZE: return "stepsize must be finite and > 0";
         case MVP_ERR_WORKSPACE: return "workspace too small or not 256-byte aligned";
         case MVP_ERR_ALGO: return "unsupported algo";
-        case MVP_ERR_ALIGN: return "misaligned buffer (tplate/rayrgba/grad_rayrgba/grad_tplate/rayaux: 16 bytes, tminmax: 8, others: 4)";
+        case MVP_ERR_ALIGN: return "misaligned buffer (tplate/grad_tplate: 16 bytes, 8 with MVP_FLAG_TPLATE_BF16; rayrgba/grad_rayrgba/rayaux/clear_grad_*: 16, tminmax: 8, others: 4)";
         case MVP_ERR_STRUCT: return "args->struct_size does not match this library's argument struct (ABI mismatch)";
         case MVP_ERR_CAMERA: return "camera.volradius must be finite and > 0";
         default: return code > 0 ? cudaGetErrorString((cudaError_t)code) : "unknown error";
@@ -2780,8 +2849,10 @@ int mvp_raymarch_forward(const mvp_forward_args *a, void *stream) {
     if (!(a->stepsize > 0.f) || !(a->stepsize < 3.0e38f)) return MVP_ERR_STEPSIZE;
     const Layout L = make_layout(a->shape);
     if (a->workspace_bytes < L.total || ((uintptr_t)a->workspace & 255)) return MVP_ERR_WORKSPACE;
-    // vector accesses: float4 (tplate, rayrgba), int4 (rayaux), float2 (tminmax); everything else is read as scalars
-    if (misaligned(a->tplate, 16) || misaligned(a->rayrgba, 16) || misaligned(a->rayaux, 16) || misaligned(a->tminmax, 8) ||
+    // vector accesses: float4 (tplate, rayrgba; a bf16 tplate 8 bytes per voxel), int4 (rayaux), float2 (tminmax); everything else
+    // is read as scalars.  The clear_grad_* buffers are zero-filled with 16-byte stores whatever the payload type.
+    const bool bf16 = (a->flags & MVP_FLAG_TPLATE_BF16) != 0;
+    if (misaligned(a->tplate, bf16 ? 8 : 16) || misaligned(a->rayrgba, 16) || misaligned(a->rayaux, 16) || misaligned(a->tminmax, 8) ||
         misaligned(a->raypos, 4) || misaligned(a->raydir, 4) || misaligned(a->primpos, 4) || misaligned(a->primrot, 4) ||
         misaligned(a->primscale, 4) || misaligned(a->raysat, 4) || misaligned(a->warp, 4) || misaligned(a->rayrgb_nchw, 4) ||
         misaligned(a->rayalpha_nchw, 4) || misaligned(a->order, 4) || misaligned(a->clear_grad_primpos, 16) ||
@@ -2796,7 +2867,7 @@ int mvp_raymarch_forward(const mvp_forward_args *a, void *stream) {
         if (rc != MVP_OK) return rc;
     }
     Params p{};
-    fill_params(p, a->shape, a->stepsize, a->fadescale, a->fadeexp, ws, L);
+    fill_params(p, a->shape, a->stepsize, a->fadescale, a->fadeexp, ws, L, bf16 ? Payload<Bf16x4>::kBytes : Payload<float4>::kBytes);
     p.pview = pview;
     p.raycam = camera ? reinterpret_cast<const float4 *>(ws + L.raycam) : nullptr;
     p.order = a->order; p.rankof = a->order ? reinterpret_cast<const int *>(ws + L.rankof) : nullptr;
@@ -2823,7 +2894,8 @@ int mvp_raymarch_forward(const mvp_forward_args *a, void *stream) {
         const size_t nk = (size_t)(pview ? a->shape.N : 1) * a->shape.K;
         float *const bufs[kClearBufs] = {a->clear_grad_primpos, a->clear_grad_primrot, a->clear_grad_primscale, a->clear_grad_tplate,
                                          a->algo == 1 ? a->clear_grad_warp : nullptr};
-        const size_t floats[kClearBufs] = {nk * 3, nk * 9, nk * 3, nk * a->shape.TD * a->shape.TH * a->shape.TW * 4,
+        // sizes in 4-byte words: a bf16 template gradient holds two channels per word
+        const size_t floats[kClearBufs] = {nk * 3, nk * 9, nk * 3, nk * a->shape.TD * a->shape.TH * a->shape.TW * (bf16 ? 2 : 4),
                                            a->algo == 1 ? nk * a->WD * a->WH * a->WW * 3 : 0};
         for (int b = 0; b < kClearBufs; ++b) {
             if (!bufs[b]) continue;
@@ -2845,22 +2917,28 @@ int mvp_raymarch_forward(const mvp_forward_args *a, void *stream) {
     const int cubic = (a->shape.TD == a->shape.TH && a->shape.TH == a->shape.TW) ? a->shape.TD : 0;
     int heavy = 0;
     if (int eh = heavy_grid(&heavy)) return eh;
-#define MVP_LAUNCH_FWD(TT, WW_)                                                                              \
+#define MVP_LAUNCH_FWD(TT, WW_, VV)                                                                          \
     do {                                                                                                     \
         if (a->raysat) {                                                                                     \
-            MVP_CARVE(MVP_FWD_CARVEOUT, render_forward_kernel<TT, true, kFastCapF, WW_>);                    \
-            MVP_LAUNCH_FAST(render_forward_kernel<TT, true, kFastCapF, WW_>);                                \
-            MVP_LAUNCH_HEAVY(render_forward_kernel<TT, true, kMaxHit, WW_>);                                 \
+            MVP_CARVE(MVP_FWD_CARVEOUT, render_forward_kernel<TT, true, kFastCapF, WW_, VV>);                \
+            MVP_LAUNCH_FAST(render_forward_kernel<TT, true, kFastCapF, WW_, VV>);                            \
+            MVP_LAUNCH_HEAVY(render_forward_kernel<TT, true, kMaxHit, WW_, VV>);                             \
         } else {                                                                                             \
-            MVP_CARVE(MVP_FWD_CARVEOUT, render_forward_kernel<TT, false, kFastCapF, WW_>);                   \
-            MVP_LAUNCH_FAST(render_forward_kernel<TT, false, kFastCapF, WW_>);                               \
-            MVP_LAUNCH_HEAVY(render_forward_kernel<TT, false, kMaxHit, WW_>);                                \
+            MVP_CARVE(MVP_FWD_CARVEOUT, render_forward_kernel<TT, false, kFastCapF, WW_, VV>);               \
+            MVP_LAUNCH_FAST(render_forward_kernel<TT, false, kFastCapF, WW_, VV>);                           \
+            MVP_LAUNCH_HEAVY(render_forward_kernel<TT, false, kMaxHit, WW_, VV>);                            \
         }                                                                                                    \
     } while (0)
-    if (a->algo == 1) MVP_LAUNCH_FWD(0, true);
-    else if (cubic == 8) MVP_LAUNCH_FWD(8, false);
-    else if (cubic == 16) MVP_LAUNCH_FWD(16, false);
-    else MVP_LAUNCH_FWD(0, false);
+#define MVP_LAUNCH_FWD_T(VV)                                                                                 \
+    do {                                                                                                     \
+        if (a->algo == 1) MVP_LAUNCH_FWD(0, true, VV);                                                       \
+        else if (cubic == 8) MVP_LAUNCH_FWD(8, false, VV);                                                   \
+        else if (cubic == 16) MVP_LAUNCH_FWD(16, false, VV);                                                 \
+        else MVP_LAUNCH_FWD(0, false, VV);                                                                   \
+    } while (0)
+    if (bf16) MVP_LAUNCH_FWD_T(Bf16x4);
+    else MVP_LAUNCH_FWD_T(float4);
+#undef MVP_LAUNCH_FWD_T
 #undef MVP_LAUNCH_FWD
     cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? MVP_OK : (int)e;
@@ -2886,7 +2964,8 @@ int mvp_raymarch_backward(const mvp_backward_args *a, void *stream) {
     if (!(a->stepsize > 0.f) || !(a->stepsize < 3.0e38f)) return MVP_ERR_STEPSIZE;
     const Layout L = make_layout(a->shape);
     if (a->workspace_bytes < L.total || ((uintptr_t)a->workspace & 255)) return MVP_ERR_WORKSPACE;
-    if (misaligned(a->tplate, 16) || misaligned(a->grad_tplate, 16) || misaligned(a->grad_rayrgba, 16) || misaligned(a->rayaux, 16) ||
+    const bool bf16 = (a->flags & MVP_FLAG_TPLATE_BF16) != 0;
+    if (misaligned(a->tplate, bf16 ? 8 : 16) || misaligned(a->grad_tplate, bf16 ? 8 : 16) || misaligned(a->grad_rayrgba, 16) || misaligned(a->rayaux, 16) ||
         misaligned(a->tminmax, 8) || misaligned(a->raypos, 4) || misaligned(a->raydir, 4) || misaligned(a->primpos, 4) ||
         misaligned(a->primrot, 4) || misaligned(a->primscale, 4) || misaligned(a->raysat, 4) || misaligned(a->grad_primpos, 4) ||
         misaligned(a->grad_primrot, 4) || misaligned(a->grad_primscale, 4) || misaligned(a->warp, 4) || misaligned(a->grad_warp, 4) ||
@@ -2904,12 +2983,13 @@ int mvp_raymarch_backward(const mvp_backward_args *a, void *stream) {
         cudaError_t z = cudaMemsetAsync(a->grad_primpos, 0, nk * 3 * sizeof(float), st);
         if (z == cudaSuccess) z = cudaMemsetAsync(a->grad_primrot, 0, nk * 9 * sizeof(float), st);
         if (z == cudaSuccess) z = cudaMemsetAsync(a->grad_primscale, 0, nk * 3 * sizeof(float), st);
-        if (z == cudaSuccess) z = cudaMemsetAsync(a->grad_tplate, 0, nk * a->shape.TD * a->shape.TH * a->shape.TW * 4 * sizeof(float), st);
+        if (z == cudaSuccess)
+            z = cudaMemsetAsync(a->grad_tplate, 0, nk * a->shape.TD * a->shape.TH * a->shape.TW * (bf16 ? Payload<Bf16x4>::kBytes : Payload<float4>::kBytes), st);
         if (z == cudaSuccess && a->algo == 1) z = cudaMemsetAsync(a->grad_warp, 0, nk * a->WD * a->WH * a->WW * 3 * sizeof(float), st);
         if (z != cudaSuccess) return (int)z;
     }
     Params p{};
-    fill_params(p, a->shape, a->stepsize, a->fadescale, a->fadeexp, ws, L);
+    fill_params(p, a->shape, a->stepsize, a->fadescale, a->fadeexp, ws, L, bf16 ? Payload<Bf16x4>::kBytes : Payload<float4>::kBytes);
     p.pview = pview;
     p.raycam = camera ? reinterpret_cast<const float4 *>(ws + L.raycam) : nullptr;
     p.raypos = a->raypos; p.raydir = a->raydir; p.tminmax = a->tminmax; p.tplate = a->tplate;
@@ -2932,16 +3012,22 @@ int mvp_raymarch_backward(const mvp_backward_args *a, void *stream) {
     const int cubic = (a->shape.TD == a->shape.TH && a->shape.TH == a->shape.TW) ? a->shape.TD : 0;
     int heavy = 0;
     if (int eh = heavy_grid(&heavy)) return eh;
-#define MVP_LAUNCH_BWD(TT, WW_)                                                                  \
+#define MVP_LAUNCH_BWD(TT, WW_, VV)                                                              \
     do {                                                                                         \
-        MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_>);                 \
-        MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_>);                             \
-        MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_>);                              \
+        MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV>);             \
+        MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV>);                         \
+        MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV>);                          \
     } while (0)
-    if (a->algo == 1) MVP_LAUNCH_BWD(0, true);
-    else if (cubic == 8) MVP_LAUNCH_BWD(8, false);
-    else if (cubic == 16) MVP_LAUNCH_BWD(16, false);
-    else MVP_LAUNCH_BWD(0, false);
+#define MVP_LAUNCH_BWD_T(VV)                                                                     \
+    do {                                                                                         \
+        if (a->algo == 1) MVP_LAUNCH_BWD(0, true, VV);                                           \
+        else if (cubic == 8) MVP_LAUNCH_BWD(8, false, VV);                                       \
+        else if (cubic == 16) MVP_LAUNCH_BWD(16, false, VV);                                     \
+        else MVP_LAUNCH_BWD(0, false, VV);                                                       \
+    } while (0)
+    if (bf16) MVP_LAUNCH_BWD_T(Bf16x4);
+    else MVP_LAUNCH_BWD_T(float4);
+#undef MVP_LAUNCH_BWD_T
 #undef MVP_LAUNCH_BWD
     cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? MVP_OK : (int)e;

@@ -71,6 +71,7 @@ _sized_init(BackwardArgs)
 FLAG_ACCEL_VALID = 1
 FLAG_ZERO_GRADS = 2
 FLAG_SHARED_PRIMS = 4
+FLAG_TPLATE_BF16 = 8
 FLAG_TEST_TINY_LISTS = 0x100
 ABI_VERSION = 8
 # layout pins, equal to the static_asserts in csrc/mvp_kernels.cu (tests/test_abi.py compares)
@@ -150,6 +151,17 @@ LIB = _load()
 def check(rc):
     if rc != 0:
         raise RuntimeError("mvpraymarch_b200: %s (code %d)" % (LIB.mvp_error_string(rc).decode(), rc))
+
+
+def tplate_flags(bf16):
+    """The flag bits that tell the raymarch calls the template's dtype: MVP_FLAG_TPLATE_BF16 for a bfloat16 template.  A library
+    built before bf16 payloads ignores unknown flags and would read the bf16 template as fp32, so the bit is set only when the
+    library reports TPLATE_BF16=1 in its build configuration."""
+    if not bf16:
+        return 0
+    if "TPLATE_BF16=1" not in LIB.mvp_build_config().decode().split():
+        raise RuntimeError("mvpraymarch_b200: this library (%s) does not support bfloat16 templates" % _build.LIB)
+    return FLAG_TPLATE_BF16
 
 
 def workspace_bytes(N, H, W, K, TD, TH, TW):

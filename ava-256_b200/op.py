@@ -8,7 +8,11 @@ everything else (mvpraymarch.py:279-292).  Differences that are deliberate:
   * no allocation or sync inside the native call (the reference cudaMalloc/cudaFree's per forward, bvh.cu:261-293);
   * the acceleration structure is a screen-space bucket list, not the BVH tensors of build_accel (:21-84);
     it is kept for backward instead of being rebuilt;
-  * 64-bit indexing (the reference overflows int32 at N*K*T^3*4 >= 2^31, primsampler.h:31-36).
+  * 64-bit indexing (the reference overflows int32 at N*K*T^3*4 >= 2^31, primsampler.h:31-36);
+  * the template may be bfloat16 (what the decoders produce under torch.autocast): it is rendered exactly as its fp32
+    widening and its gradient is bfloat16, accumulated in bf16 by the backward kernel.  `mvpraymarch` widens bfloat16
+    primpos / primrot / primscale / warp to fp32 before the op (exact; autograd casts their gradients back).  The reference
+    reads a half-precision template as fp32 without checking its dtype (mvpraymarch.cpp:250-272).
 """
 import ctypes
 
@@ -30,13 +34,21 @@ def _aligned(t, nbytes):
     return t
 
 
-def _check_f32_cuda(name, t):
+def _check_f32_cuda(name, t, allow_bf16=False):
     if not t.is_cuda:
         raise RuntimeError("%s must be a CUDA tensor" % name)          # mvpraymarch.cpp:102
     if not t.is_contiguous():
         raise RuntimeError("%s must be contiguous" % name)             # mvpraymarch.cpp:103
-    if t.dtype != torch.float32:
+    if allow_bf16:
+        if t.dtype not in (torch.float32, torch.bfloat16):
+            raise RuntimeError("%s must be float32 or bfloat16, got %s" % (name, t.dtype))
+    elif t.dtype != torch.float32:
         raise RuntimeError("%s must be float32" % name)
+
+
+def _widen_bf16(t):
+    """A bfloat16 tensor as fp32 (exact); anything else unchanged, so that other dtypes still meet the op's dtype check."""
+    return t.float() if t is not None and t.dtype == torch.bfloat16 else t
 
 
 class MVPRaymarch(Function):
@@ -74,9 +86,12 @@ class MVPRaymarch(Function):
         assert template.is_contiguous() and template.dim() == 6 and template.size(-1) == 4, \
             "channels-last template [N,K,TD,TH,TW,4] required (the reference sampler is always channels-last, primsampler.h:16)"
         for name, t in (("raypos", raypos), ("raydir", raydir), ("tminmax", tminmax), ("primpos", primpos),
-                        ("primrot", primrot), ("primscale", primscale), ("template", template)):
+                        ("primrot", primrot), ("primscale", primscale)):
             if t is not None:
                 _check_f32_cuda(name, t)
+        _check_f32_cuda("template", template, allow_bf16=True)
+        bf16 = template.dtype == torch.bfloat16                        # MVP_FLAG_TPLATE_BF16: rendered as template.float()
+        tflags = _lib.tplate_flags(bf16)
         if warp is not None:                                           # mvpraymarch.py:124
             assert warp.is_contiguous() and warp.dim() == 6 and warp.size(-1) == 3, \
                 "channels-last warp field [N,K,WD,WH,WW,3] required"
@@ -103,7 +118,7 @@ class MVPRaymarch(Function):
         if warp is not None:
             assert warp.shape[:2] == (NP, K), "warp disagrees with the primitives on [N,K]"
         shared = NP == 1 and N > 1
-        template, tminmax = _aligned(template, 16), _aligned(tminmax, 8)
+        template, tminmax = _aligned(template, 8 if bf16 else 16), _aligned(tminmax, 8)
         with torch.cuda.device(dev):
             wsbytes = _lib.workspace_bytes(N, H, W, K, TD, TH, TW)
             workspace = torch.empty(wsbytes, dtype=torch.uint8, device=dev)
@@ -122,7 +137,7 @@ class MVPRaymarch(Function):
             a = _lib.ForwardArgs()
             a.shape = _lib.Shape(N, H, W, K, TD, TH, TW)
             a.stepsize, a.fadescale, a.fadeexp = float(stepsize), float(options["fadescale"]), float(options["fadeexp"])
-            a.flags = _lib.FLAG_SHARED_PRIMS if shared else 0
+            a.flags = (_lib.FLAG_SHARED_PRIMS if shared else 0) | tflags
             a.raypos, a.raydir, a.tminmax = _ptr(raypos), _ptr(raydir), _ptr(tminmax)
             if camera is not None:
                 a.camera = _lib.Camera(_ptr(viewpos), _ptr(viewrot), _ptr(focal), _ptr(princpt), float(volradius), 0)
@@ -160,6 +175,7 @@ class MVPRaymarch(Function):
             ctx.options = options
             ctx.stepsize = float(stepsize)
             ctx.shared = shared
+            ctx.tflags = tflags
         if planes:
             return rayrgb, rayalpha
         return rayrgba
@@ -193,7 +209,8 @@ class MVPRaymarch(Function):
             a = _lib.BackwardArgs()
             a.shape = _lib.Shape(N, H, W, K, TD, TH, TW)
             a.stepsize, a.fadescale, a.fadeexp = ctx.stepsize, float(options["fadescale"]), float(options["fadeexp"])
-            a.flags = _lib.FLAG_ACCEL_VALID | (0 if fresh else _lib.FLAG_ZERO_GRADS) | (_lib.FLAG_SHARED_PRIMS if ctx.shared else 0)
+            a.flags = _lib.FLAG_ACCEL_VALID | (0 if fresh else _lib.FLAG_ZERO_GRADS) | (_lib.FLAG_SHARED_PRIMS if ctx.shared else 0) | \
+                ctx.tflags
             a.raypos, a.raydir, a.tminmax = _ptr(raypos), _ptr(raydir), _ptr(tminmax)
             if ctx.camera is not None:
                 viewpos, viewrot, focal, princpt, volradius = ctx.camera[:5]
@@ -326,6 +343,9 @@ def mvpraymarch(
         primpos = primtransf[:, :, 0, :].contiguous()
         primrot = primtransf[:, :, 1:4, :].contiguous()
         primscale = primtransf[:, :, 4, :].contiguous()
+    # under torch.autocast the decoders hand over bfloat16 transforms: widened here, outside the autograd Function, so that
+    # torch casts their gradients back (the template itself goes to the kernels as bfloat16)
+    primpos, primrot, primscale, warp = (_widen_bf16(t) for t in (primpos, primrot, primscale, warp))
     order = None
     if usebvh != "fixedorder":
         # Morton order of the centres as an indirection inside the kernels (C-ABI `order`): nothing is gathered or copied

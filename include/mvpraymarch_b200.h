@@ -28,7 +28,8 @@
  *
  * Conventions (same ownership model as the reference: the caller owns every buffer, outputs are written in
  * place; unlike the reference nothing is allocated inside and everything runs on the caller's stream):
- *   - all pointers are DEVICE pointers to contiguous fp32 (or int32) arrays; no torch types;
+ *   - all pointers are DEVICE pointers to contiguous fp32 (or int32) arrays, except the template and its gradient, which may be
+ *     bfloat16 (MVP_FLAG_TPLATE_BF16); no torch types;
  *   - `stream` is a cudaStream_t passed as void*;
  *   - return value: 0 = ok, < 0 = invalid argument (MVP_ERR_*), > 0 = a cudaError_t from the launch;
  *   - thread-safe and re-entrant: no global state.
@@ -57,8 +58,9 @@ extern "C" {
 #define MVP_ERR_STEPSIZE (-3)  /* stepsize must be finite and > 0 */
 #define MVP_ERR_WORKSPACE (-4) /* workspace too small or misaligned (256 B) */
 #define MVP_ERR_ALGO (-5)      /* algo must be 0 (no warp field) or 1 (warp field, primsampler.h:53-58) */
-#define MVP_ERR_ALIGN (-6)     /* a vector-accessed buffer is misaligned: tplate, rayrgba, grad_rayrgba, grad_tplate, rayaux
-                                * need 16 bytes, tminmax 8, everything else 4 */
+#define MVP_ERR_ALIGN (-6)     /* a vector-accessed buffer is misaligned: tplate, rayrgba, grad_rayrgba, grad_tplate, rayaux,
+                                * clear_grad_* need 16 bytes (tplate, grad_tplate 8 with MVP_FLAG_TPLATE_BF16), tminmax 8,
+                                * everything else 4 */
 #define MVP_ERR_STRUCT (-7)    /* args->struct_size != sizeof(the struct this library was built with) */
 #define MVP_ERR_CAMERA (-8)    /* camera.volradius must be finite and > 0 */
 
@@ -74,6 +76,12 @@ typedef struct mvp_shape {
                                  * ONE that all N views share: [1,K,...] instead of [N,K,...] (SURVEY.md section 8e
                                  * "optional fast path"); gradients of all views accumulate into the one set.  Must be the
                                  * same in mvp_build_accel / forward / backward calls that share a workspace. */
+#define MVP_FLAG_TPLATE_BF16 8u  /* forward and backward: tplate, grad_tplate and clear_grad_tplate point to bfloat16, not fp32
+                                 * (same [N,K,TD,TH,TW,4] channels-last layout, 8 bytes per voxel; tplate and grad_tplate 8-byte
+                                 * aligned, clear_grad_tplate 16).  The output is exactly that of the fp32 kernels on the widened
+                                 * template; grad_tplate is accumulated in bf16 (round to nearest even per reduction).  Everything
+                                 * else stays fp32.  Must be the same in a forward and the backward that follows it.  The library
+                                 * supports it iff mvp_build_config() lists TPLATE_BF16=1 (an older one ignores the bit). */
 #define MVP_FLAG_TEST_TINY_LISTS 0x100u /* test hook: forward keeps at most 16 saved tile-list entries per view, so almost
                                  * every tile takes the backward's rebuild path */
 
