@@ -12,6 +12,7 @@
 #include <cuda_runtime.h>  // float4 / make_float4 on host and device
 #include <stddef.h>
 #include <stdint.h>
+#include <string.h>
 
 #ifdef __CUDACC__
 #define MVP_HD __host__ __device__ __forceinline__
@@ -184,7 +185,7 @@ struct PayloadArgs {
     int32_t hb, wb, B;
     float rgb_scale, rgb_bias;
     const float *tex, *opacity; // forward in
-    float *tplate;              // forward out
+    float *tplate;              // forward out (bf16 texels in the _bf16 bodies below, as are the next two)
     const float *tplate_in;     // backward in (relu mask)
     const float *grad_tplate;   // backward in
     float *grad_tex, *grad_opacity; // backward out
@@ -249,6 +250,110 @@ MVP_HD void payload_bwd(const PayloadArgs &a, size_t e) {
         g1[v] = t.y > 0.f ? MVP_MUL(g.y, a.rgb_scale) : 0.f;
         g2[v] = t.z > 0.f ? MVP_MUL(g.z, a.rgb_scale) : 0.f;
         go[v] = t.w > 0.f ? g.w : 0.f;
+    }
+    store<V>(a.grad_tex + ix.tex_off, g0);
+    store<V>(a.grad_tex + ix.tex_off + ix.plane, g1);
+    store<V>(a.grad_tex + ix.tex_off + 2 * ix.plane, g2);
+    store<V>(a.grad_opacity + ix.opa_off, go);
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// bfloat16 forms (mvp_assemble_payload_*_bf16, mvp_sum_views_bf16).  A bf16 texel is 8 bytes, two 32-bit words holding
+// channel pairs: word 0 = ch0 | ch1 << 16, word 1 = ch2 | ch3 << 16 (little endian: channel 0 first), the layout the
+// render kernels read with MVP_FLAG_TPLATE_BF16.  The PayloadArgs pointers tplate / tplate_in / grad_tplate then point to
+// bf16 data.
+//   forward:  the fp32 arithmetic above unchanged, then each channel rounded once to bf16 (nearest even, subnormals kept,
+//             NaN stays NaN): bit-identical to assemble_payload_ref(tex, opacity, B).to(torch.bfloat16).  16 B in + 8 B out
+//             per texel.
+//   backward: the bf16 gradient widened exactly, masked where the bf16 template is > 0, times rgb_scale (one fp32 rounding):
+//             bit-identical to eager autograd through assemble_payload_ref(...).to(torch.bfloat16) for the same bf16 gradient,
+//             with one exception.  An fp32 relu output in (0, 2^-134] rounds to bf16 +0 (half the smallest bf16 subnormal,
+//             2^-133, ties to even), so the mask read from the bf16 template is 0 there while eager's, taken on the fp32 relu
+//             output, is 1.  16 B in + 16 B out per texel.
+// ------------------------------------------------------------------------------------------------------------------
+MVP_HD float bits_to_float(uint32_t u) {
+#ifdef __CUDA_ARCH__
+    return __uint_as_float(u);
+#else
+    float f;
+    memcpy(&f, &u, 4);
+    return f;
+#endif
+}
+
+// Two fp32 values as one bf16 pair, `lo` in the low half; each rounded to nearest even (cvt.rn.bf16x2.f32 on the device).
+MVP_HD uint32_t pack_bf16x2(float lo, float hi) {
+#ifdef __CUDA_ARCH__
+    uint32_t d;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));   // first source -> upper half
+    return d;
+#else
+    const auto rn = [](float x) -> uint32_t {
+        uint32_t u;
+        memcpy(&u, &x, 4);
+        if ((u & 0x7fffffffu) > 0x7f800000u) return (u >> 16) | 0x40u;    // NaN: quiet, sign and top payload kept
+        return (u + 0x7fffu + ((u >> 16) & 1u)) >> 16;
+    };
+    return rn(lo) | (rn(hi) << 16);
+#endif
+}
+// Exact widening of the low / high bf16 of a pair.
+MVP_HD float bf16_lo(uint32_t w) { return bits_to_float(w << 16); }
+MVP_HD float bf16_hi(uint32_t w) { return bits_to_float(w & 0xffff0000u); }
+
+// The 2V words of V consecutive bf16 texels (V = 4: two 16-byte accesses, 16-byte alignment; V = 1: one 8-byte access).
+template <int V>
+MVP_HD void load_words(const uint32_t *p, uint32_t (&w)[2 * V]) {
+    if constexpr (V == 4) {
+        const uint4 a = MVP_LDG(reinterpret_cast<const uint4 *>(p)), b = MVP_LDG(reinterpret_cast<const uint4 *>(p) + 1);
+        w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
+    } else {
+        const uint2 a = MVP_LDG(reinterpret_cast<const uint2 *>(p));
+        w[0] = a.x; w[1] = a.y;
+    }
+}
+template <int V>
+MVP_HD void store_words(uint32_t *p, const uint32_t (&w)[2 * V]) {
+    if constexpr (V == 4) {
+        reinterpret_cast<uint4 *>(p)[0] = make_uint4(w[0], w[1], w[2], w[3]);
+        reinterpret_cast<uint4 *>(p)[1] = make_uint4(w[4], w[5], w[6], w[7]);
+    } else {
+        *reinterpret_cast<uint2 *>(p) = make_uint2(w[0], w[1]);
+    }
+}
+
+template <int V, int BT>
+MVP_HD void payload_fwd_bf16(const PayloadArgs &a, size_t e) {
+    const PayloadIndex ix = payload_index<V, BT>(a, e);
+    float c0[V], c1[V], c2[V], o[V];
+    load<V>(a.tex + ix.tex_off, c0);
+    load<V>(a.tex + ix.tex_off + ix.plane, c1);
+    load<V>(a.tex + ix.tex_off + 2 * ix.plane, c2);
+    load<V>(a.opacity + ix.opa_off, o);
+    uint32_t w[2 * V];
+#pragma unroll
+    for (int v = 0; v < V; ++v) {
+        w[2 * v] = pack_bf16x2(relu_keep_nan(MVP_ADD(MVP_MUL(c0[v], a.rgb_scale), a.rgb_bias)),
+                               relu_keep_nan(MVP_ADD(MVP_MUL(c1[v], a.rgb_scale), a.rgb_bias)));
+        w[2 * v + 1] = pack_bf16x2(relu_keep_nan(MVP_ADD(MVP_MUL(c2[v], a.rgb_scale), a.rgb_bias)), relu_keep_nan(o[v]));
+    }
+    store_words<V>(reinterpret_cast<uint32_t *>(a.tplate) + 2 * ix.slab_off, w);
+}
+
+template <int V, int BT>
+MVP_HD void payload_bwd_bf16(const PayloadArgs &a, size_t e) {
+    const PayloadIndex ix = payload_index<V, BT>(a, e);
+    uint32_t t[2 * V], g[2 * V];
+    load_words<V>(reinterpret_cast<const uint32_t *>(a.tplate_in) + 2 * ix.slab_off, t);
+    load_words<V>(reinterpret_cast<const uint32_t *>(a.grad_tplate) + 2 * ix.slab_off, g);
+    float g0[V], g1[V], g2[V], go[V];
+#pragma unroll
+    for (int v = 0; v < V; ++v) {
+        const uint32_t t01 = t[2 * v], t23 = t[2 * v + 1], g01 = g[2 * v], g23 = g[2 * v + 1];
+        g0[v] = bf16_lo(t01) > 0.f ? MVP_MUL(bf16_lo(g01), a.rgb_scale) : 0.f;
+        g1[v] = bf16_hi(t01) > 0.f ? MVP_MUL(bf16_hi(g01), a.rgb_scale) : 0.f;
+        g2[v] = bf16_lo(t23) > 0.f ? MVP_MUL(bf16_lo(g23), a.rgb_scale) : 0.f;
+        go[v] = bf16_hi(t23) > 0.f ? bf16_hi(g23) : 0.f;
     }
     store<V>(a.grad_tex + ix.tex_off, g0);
     store<V>(a.grad_tex + ix.tex_off + ix.plane, g1);

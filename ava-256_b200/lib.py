@@ -83,7 +83,8 @@ EXPORTS = ("mvp_abi_version", "mvp_build_config", "mvp_error_string", "mvp_works
            "mvp_composite_forward", "mvp_composite_backward", "mvp_assemble_payload_forward",
            "mvp_assemble_payload_backward", "mvp_debug_saved_tiles", "mvp_debug_tileclk_offset", "mvp_debug_heavy_offset",
            "mvp_compute_morton",
-           "mvp_expand_views", "mvp_sum_views")
+           "mvp_expand_views", "mvp_sum_views", "mvp_assemble_payload_forward_bf16", "mvp_assemble_payload_backward_bf16",
+           "mvp_sum_views_bf16")
 
 
 def _load():
@@ -132,6 +133,12 @@ def _load():
     lib.mvp_assemble_payload_forward.argtypes = [ctypes.c_int32] * 4 + [c_f] * 2 + [ctypes.c_float] * 2 + [c_f] * 2
     lib.mvp_assemble_payload_backward.restype = ctypes.c_int
     lib.mvp_assemble_payload_backward.argtypes = [ctypes.c_int32] * 4 + [c_f] * 2 + [ctypes.c_float] + [c_f] * 3
+    lib.mvp_assemble_payload_forward_bf16.restype = ctypes.c_int
+    lib.mvp_assemble_payload_forward_bf16.argtypes = [ctypes.c_int32] * 4 + [c_f] * 2 + [ctypes.c_float] * 2 + [c_f] * 2
+    lib.mvp_assemble_payload_backward_bf16.restype = ctypes.c_int
+    lib.mvp_assemble_payload_backward_bf16.argtypes = [ctypes.c_int32] * 4 + [c_f] * 2 + [ctypes.c_float] + [c_f] * 3
+    lib.mvp_sum_views_bf16.restype = ctypes.c_int
+    lib.mvp_sum_views_bf16.argtypes = [c_f, c_f, ctypes.c_size_t, ctypes.c_int32, ctypes.c_int32, c_f]
     lib.mvp_debug_heavy_offset.restype = ctypes.c_size_t
     lib.mvp_debug_heavy_offset.argtypes = [ctypes.POINTER(Shape)]
     lib.mvp_forward_launch_count.restype = ctypes.c_int
@@ -162,6 +169,13 @@ def tplate_flags(bf16):
     if "TPLATE_BF16=1" not in LIB.mvp_build_config().decode().split():
         raise RuntimeError("mvpraymarch_b200: this library (%s) does not support bfloat16 templates" % _build.LIB)
     return FLAG_TPLATE_BF16
+
+
+def require_epilogue_bf16():
+    """Raise unless the library has the bf16 payload hand-off and view sum (mvp_assemble_payload_*_bf16, mvp_sum_views_bf16),
+    which it reports as EPILOGUE_BF16=1 in its build configuration."""
+    if "EPILOGUE_BF16=1" not in LIB.mvp_build_config().decode().split():
+        raise RuntimeError("mvpraymarch_b200: this library (%s) does not support bfloat16 payload hand-off" % _build.LIB)
 
 
 def workspace_bytes(N, H, W, K, TD, TH, TW):

@@ -1,6 +1,7 @@
 """Multi-GPU plumbing of the path (SURVEY.md section 8e): views shard over ranks with no data-path collective in
 forward; when the views of a step share one subject's primitives, the per-view primitive gradients are summed locally
-and all-reduced once per step (one flat fp32 buffer: template, primpos, primrot, primscale)."""
+and all-reduced once per step (one flat fp32 buffer: template, primpos, primrot, primscale).  A bf16 template gradient is
+summed over the views straight into the fp32 buffer (exact widening, fp32 accumulation); the all-reduce stays fp32."""
 import torch
 import torch.distributed as dist
 
@@ -26,13 +27,14 @@ def rank_views(n_views, rank, world, interleave=True):
 
 
 def _sum_views(p, out):
-    """out[...] = sum over the local views of p [nv, ...]: the library's one-pass kernel on the GPU (`mvp_sum_views`), torch.sum for
-    host tensors (the world-size-2 gloo tests of this module's logic run on the CPU)."""
+    """out[...] = sum over the local views of p [nv, ...]: the library's one-pass kernel on the GPU (`mvp_sum_views`, or
+    `mvp_sum_views_bf16` for a bf16 p and an fp32 out), torch.sum for host tensors (the world-size-2 gloo tests of this module's
+    logic run on the CPU), which widens a bf16 p to out's dtype first."""
     if p.is_cuda:
         from .payload import sum_views
         sum_views(p, out)
     else:
-        torch.sum(p.reshape(p.shape[0], -1), dim=0, out=out)
+        torch.sum(p.reshape(p.shape[0], -1).to(out.dtype), dim=0, out=out)
 
 
 def flat_grad_numel(K, TD, TH, TW):
@@ -43,12 +45,13 @@ def reduce_primitive_grads(grad_template, grad_primpos, grad_primrot, grad_prims
     """Sum per-view gradients [nv, ...] over the local views into `flat` and all-reduce it (if a process group is up).
 
     Returns (flat, views) where views = (g_template [K,TD,TH,TW,4], g_primpos [K,3], g_primrot [K,3,3], g_primscale [K,3])
-    are views into flat."""
+    are views into flat.  A bf16 grad_template is summed into an fp32 flat buffer."""
     parts = (grad_template, grad_primpos, grad_primrot, grad_primscale)
     nv = grad_template.shape[0]
     total = sum(p[0].numel() for p in parts)
     if flat is None:
-        flat = torch.empty(total, dtype=grad_template.dtype, device=grad_template.device)
+        dtype = torch.float32 if grad_template.dtype == torch.bfloat16 else grad_template.dtype
+        flat = torch.empty(total, dtype=dtype, device=grad_template.device)
     assert flat.numel() == total
     o = 0
     views = []
@@ -67,7 +70,8 @@ class GradReducer:
     path: the rank's per-view gradients are summed into one of two flat buffers on the compute stream and the NCCL
     all-reduce of that buffer is launched asynchronously (NCCL's own stream), so it overlaps whatever the caller enqueues
     next -- normally the next step's forward.  A buffer is waited for only when it is about to be reused, when the caller
-    asks for its contents (`wait`), or at `finish()`.
+    asks for its contents (`wait`), or at `finish()`.  A bf16 template gradient is summed into the fp32 buffer with fp32
+    accumulation.
 
         red = GradReducer(K, TD, TH, TW, device)
         for step ...:

@@ -29,7 +29,7 @@
  * Conventions (same ownership model as the reference: the caller owns every buffer, outputs are written in
  * place; unlike the reference nothing is allocated inside and everything runs on the caller's stream):
  *   - all pointers are DEVICE pointers to contiguous fp32 (or int32) arrays, except the template and its gradient, which may be
- *     bfloat16 (MVP_FLAG_TPLATE_BF16); no torch types;
+ *     bfloat16 (MVP_FLAG_TPLATE_BF16, and the bf16 forms mvp_assemble_payload_*_bf16 / mvp_sum_views_bf16); no torch types;
  *   - `stream` is a cudaStream_t passed as void*;
  *   - return value: 0 = ok, < 0 = invalid argument (MVP_ERR_*), > 0 = a cudaError_t from the launch;
  *   - thread-safe and re-entrant: no global state.
@@ -224,6 +224,16 @@ int mvp_assemble_payload_forward(int32_t N, int32_t hb, int32_t wb, int32_t B, c
 /* Adjoint: grad_tex / grad_opacity (same shapes as tex / opacity) are written; `tplate` is the forward output (relu mask). */
 int mvp_assemble_payload_backward(int32_t N, int32_t hb, int32_t wb, int32_t B, const float *tplate, const float *grad_tplate,
                                   float rgb_scale, float *grad_tex, float *grad_opacity, void *stream);
+/* The same with a bfloat16 template (the layout MVP_FLAG_TPLATE_BF16 reads: 8 bytes per texel).  Forward: the fp32 values above,
+ * each rounded once to bf16 (nearest even; NaN stays NaN).  Backward: grad_tplate is bf16, widened exactly, masked where the bf16
+ * tplate is > 0 and multiplied by rgb_scale in fp32; grad_tex / grad_opacity stay fp32.  A relu output in (0, 2^-134] rounds to
+ * bf16 zero, so its gradient is masked, where the fp32 chain would pass it.  tplate and grad_tplate need 8-byte alignment (the
+ * 16-byte vector variant is taken when they, tex / opacity or grad_tex / grad_opacity are 16-byte aligned and B % 4 == 0).
+ * The library supports these iff mvp_build_config() lists EPILOGUE_BF16=1. */
+int mvp_assemble_payload_forward_bf16(int32_t N, int32_t hb, int32_t wb, int32_t B, const float *tex, const float *opacity,
+                                      float rgb_scale, float rgb_bias, void *tplate, void *stream);
+int mvp_assemble_payload_backward_bf16(int32_t N, int32_t hb, int32_t wb, int32_t B, const void *tplate, const void *grad_tplate,
+                                       float rgb_scale, float *grad_tex, float *grad_opacity, void *stream);
 
 /* One subject's primitives materialised per view (what the decoders' batch dimension is in models/autoencoder.py:214-233
  * when all items of a batch show the same subject): dst[v, i] = src[i] for v < n_views, i < count floats.  One pass of
@@ -234,6 +244,11 @@ int mvp_expand_views(const float *src, float *dst, size_t count, int32_t n_views
  * subject's primitives, their gradients are summed before the one all-reduce): dst[i] = sum over v < n_views of src[v, i], added
  * in view order (deterministic), one pass over the per-view gradients.  Same alignment rule as mvp_expand_views; n_views >= 1. */
 int mvp_sum_views(const float *src, float *dst, size_t count, int32_t n_views, void *stream);
+/* The same over bfloat16 views: src [n_views, count] bf16, each value widened exactly and added in fp32 in view order, so an fp32
+ * dst (dst_bf16 = 0) equals mvp_sum_views of the widened source bit for bit; a bf16 dst (dst_bf16 != 0) gets that sum rounded
+ * once (nearest even).  src 2-byte aligned, dst 4 (fp32) or 2 (bf16); 16-byte accesses when count % 8 == 0 and both pointers
+ * are 16-byte aligned.  A bf16 tensor is expanded with mvp_expand_views as 4-byte words (count / 2, even counts). */
+int mvp_sum_views_bf16(const void *src, void *dst, size_t count, int32_t n_views, int32_t dst_bf16, void *stream);
 
 /* Test / diagnostics helper (host only, no device work): given a HOST copy of a workspace that a gradient-mode forward
  * has filled, counts the tiles whose slab list the forward saved for the backward (`saved`, lists with >= 1 entry) and the
