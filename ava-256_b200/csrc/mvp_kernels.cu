@@ -1055,6 +1055,10 @@ struct Params {
     // floats, and float4s per warp of the fast render launch
     float *clr[kClearBufs];
     unsigned long long clrn[kClearBufs], clrper[kClearBufs];
+    // mvp_raymarch_backward_rays: per-ray gradients [N,H,W,3] / [N,H,W,3] / [N,H,W,2], written once per ray (kRayGrad kernels only;
+    // appended last so that the parameter offsets of every other kernel stay what they were)
+    float *g_raypos, *g_raydir;
+    float2 *g_tminmax;
 };
 
 #if defined(MVP_CPU_EMUL) && defined(MVP_EMUL_STATS)
@@ -1933,6 +1937,35 @@ struct __align__(16) BwdWarpSmem {   // per-warp shared state of the backward ke
 #endif
 };
 
+// The backward that also returns the ray gradients (kRayGrad) keeps per warp:
+//   rj: the lattice step j of each queued sample, beside its record in the sample queue q (same slot);
+//   rs: the current slab's sums over the samples of each OWNER lane's ray, in slab coordinates: sum dL/dy, sum j dL/dy
+//       (j = the sample's lattice step); added to by whichever lane computes a sample, read and cleared by the owner per slab;
+//   ra: the ray's totals in world coordinates, sum dL/dx and sum j dL/dx, dL/dx = R (s * dL/dy) once per lane and slab.
+template <int CAP>
+struct __align__(16) BwdWarpSmemRays : BwdWarpSmem<CAP> {
+    int rj[kRing];
+    float rs[6 * 32];
+    float ra[6 * 32];
+};
+template <int CAP, bool kRayGrad> struct BwdSmemOf { using type = BwdWarpSmem<CAP>; };
+template <int CAP> struct BwdSmemOf<CAP, true> { using type = BwdWarpSmemRays<CAP>; };
+
+// kRayGrad: this lane's ray gradients, one write per ray at the end of its tile (pixels outside the image write nothing).  With
+// P = sum_j dL/dx_j and J = sum_j j dL/dx_j over the ray's samples x_j = o + d (tmin + j dt):
+//   dL/d raypos = P,   dL/d raydir = tmin P + dt J,   dL/d tminmax = (<d, P>, 0).
+__device__ __forceinline__ void store_ray_grads(const Params &p, int n, int tx, int ty, int lane, float P0, float P1, float P2, float J0,
+                                                float J1, float J2, float tmin, float dx, float dy, float dz) {
+    const int px = tx * kTileW + (lane & 7), py = ty * kTileH + (lane >> 3);
+    if (px >= p.W || py >= p.H) return;
+    const size_t r = ((size_t)n * p.H + py) * p.W + px;
+    p.g_raypos[r * 3 + 0] = P0; p.g_raypos[r * 3 + 1] = P1; p.g_raypos[r * 3 + 2] = P2;
+    p.g_raydir[r * 3 + 0] = __fmaf_rn(p.dt, J0, tmin * P0);
+    p.g_raydir[r * 3 + 1] = __fmaf_rn(p.dt, J1, tmin * P1);
+    p.g_raydir[r * 3 + 2] = __fmaf_rn(p.dt, J2, tmin * P2);
+    p.g_tminmax[r] = make_float2(__fmaf_rn(dz, P2, __fmaf_rn(dy, P1, dx * P0)), 0.f);
+}
+
 // The slab record from shared memory through loads the compiler can neither hoist nor keep alive: the caller decides where the
 // 15 values are live.
 __device__ __forceinline__ Prim load_rec_shared(const float4 *rec) {
@@ -1954,13 +1987,26 @@ __device__ __forceinline__ Prim load_rec_shared(const float4 *rec) {
     return q;
 }
 
-template <int T, int CAP, bool kWarp, typename V>
+template <int CAP, bool kRayGrad>
+__device__ __forceinline__ float *ray_sums(BwdWarpSmem<CAP> *S, bool totals) {
+    if constexpr (kRayGrad) return totals ? static_cast<BwdWarpSmemRays<CAP> *>(S)->ra : static_cast<BwdWarpSmemRays<CAP> *>(S)->rs;
+    else return nullptr;
+}
+template <int CAP, bool kRayGrad>
+__device__ __forceinline__ int *ray_steps(BwdWarpSmem<CAP> *S) {
+    if constexpr (kRayGrad) return static_cast<BwdWarpSmemRays<CAP> *>(S)->rj;
+    else return nullptr;
+}
+
+template <int T, int CAP, bool kWarp, typename V, bool kRayGrad>
 __device__ __forceinline__ bool backward_tile(const Params &p, const int n, const int tx, const int ty, const int lane, BwdWarpSmem<CAP> *const S) {
     int *const sk = S->k, *const siv = S->iv;
     RowEntry *const sstage = S->stage;
     unsigned long long *const sbar = S->bar;
     float4 *const sq = S->q;
     float *const sray = S->ray;   // per-ray adjoint constants: dL.xyzw, saturation colour + flag, alpha before saturation
+    float *const srs = ray_sums<CAP, kRayGrad>(S, false), *const sra = ray_sums<CAP, kRayGrad>(S, true);   // kRayGrad only
+    int *const srj = ray_steps<CAP, kRayGrad>(S);                                                         // kRayGrad only
 
     const float rdt = fast_rcp(p.dt);
     TileCtx c;
@@ -1973,7 +2019,10 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
 #endif
     if (have == 0 && !build_tile_list<CAP, false>(p, rdt, n, tx, ty, lane, c, sk, siv, sstage, sbar, t0, xb, yb, zb, r1e, j0)) return false;
     const int nl = c.nl;
-    if (nl == 0) return true;
+    if (nl == 0) {
+        if (kRayGrad) store_ray_grads(p, n, tx, ty, lane, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f);
+        return true;
+    }
 
     const int px = tx * kTileW + (lane & 7), py = ty * kTileH + (lane >> 3);
     const size_t r = ((size_t)n * p.H + min(py, p.H - 1)) * p.W + min(px, p.W - 1);
@@ -1999,6 +2048,10 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
         pr_[4 * 32 + lane] = hassat ? rs0 : 0.f; pr_[5 * 32 + lane] = hassat ? rs1 : 0.f; pr_[6 * 32 + lane] = hassat ? rs2 : 0.f;
         pr_[7 * 32 + lane] = hassat ? 1.f : 0.f;
         pr_[8 * 32 + lane] = __int_as_float(aux.z);      // alpha before the saturating sample
+        if (kRayGrad) {
+#pragma unroll
+            for (int f = 0; f < 6; ++f) { srs[f * 32 + lane] = 0.f; sra[f * 32 + lane] = 0.f; }
+        }
         __syncwarp();
     }
 
@@ -2008,7 +2061,10 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
     const float foff = (float)c.off;
     const int wlast = __reduce_max_sync(0xffffffffu, mlast);
     const int wfirst = __reduce_min_sync(0xffffffffu, ms);
-    if (wlast < wfirst || wfirst >= kBig) return true;
+    if (wlast < wfirst || wfirst >= kBig) {
+        if (kRayGrad) store_ray_grads(p, n, tx, ty, lane, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f);
+        return true;
+    }
 
     const float4 *packn = p.pack + (size_t)(n * p.pview) * p.K * 4;
     const size_t slabsz = (size_t)p.TD * p.TH * p.TW;   // (a compile-time T^3 here makes the compiler keep slab addresses in registers: 64 B of spills)
@@ -2158,6 +2214,8 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                 bool touched = false;
                 // the step at which this lane's walk of this slab meets the ray's saturating sample (-1: never)
                 const int isat_i = (rank == L_RANKSAT) ? (L_MSAT - la) : -1;
+                // kRayGrad: lattice step of the walk's first candidate; sample i is at step jb + i (a full int, beside the queue)
+                const int jb = kRayGrad ? la + c.off : 0;
                 // carry the lane's position from the chunk base (step max(cs, ms)) to its first candidate step
                 float x = L_XB, y = L_YB, z = L_ZB;
                 {
@@ -2201,6 +2259,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                                 const int pos = (qhead + qn + __popc(vm & ((1u << lane) - 1u))) & (kRing - 1);
                                 const bool issat = (i == isat_i);
                                 ring[pos] = make_float4(xm, ym, zm, __int_as_float(lane | (issat ? 256 : 0)));
+                                if (kRayGrad) srj[pos] = jb + i;
                             }
                             qn += __popc(vm);
 #if defined(MVP_CPU_EMUL) && defined(MVP_EMUL_STATS)
@@ -2224,6 +2283,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         const int cnt = min(qn, 32);
                         const bool act = lane < cnt;
                         const float4 rec = ring[(qhead + (act ? lane : 0)) & (kRing - 1)];
+                        const int jrec = kRayGrad ? srj[(qhead + (act ? lane : 0)) & (kRing - 1)] : 0;
                         qhead = (qhead + cnt) & (kRing - 1);
                         qn -= cnt;
                         __syncwarp();
@@ -2414,6 +2474,13 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         }
                         gy0 += ((float)(p.WW - 1) * 0.5f) * h0; gy1 += ((float)(p.WH - 1) * 0.5f) * h1; gy2 += ((float)(p.WD - 1) * 0.5f) * h2;
                         }
+                        if (kRayGrad) {
+                            // this sample's dL/dy and j dL/dy into its owner's sums (shared-memory atomics: lanes of a batch share owners)
+                            const float jf = (float)jrec;
+                            float *o = srs + owner;
+                            atomicAdd(o + 0 * 32, gy0); atomicAdd(o + 1 * 32, gy1); atomicAdd(o + 2 * 32, gy2);
+                            atomicAdd(o + 3 * 32, jf * gy0); atomicAdd(o + 4 * 32, jf * gy1); atomicAdd(o + 5 * 32, jf * gy2);
+                        }
                         // ---- primtransf.h:155-179, accumulated in factored form ----
 #if MVP_BWD_LANESMEM
                         L_GX(0) = L_GX(0) + xm * gy0; L_GX(1) = L_GX(1) + xm * gy1; L_GX(2) = L_GX(2) + xm * gy2;
@@ -2439,6 +2506,22 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                 for (int i = 0; i < 9; ++i) gx[i] = L_GX(i);
                 gsum[0] = L_GX(9); gsum[1] = L_GX(10); gsum[2] = L_GX(11);
 #endif
+                if (kRayGrad) {
+                    // the owner's slab sums to world coordinates, dL/dx = R (s * dL/dy), into the ray's totals; cleared for the next slab
+                    __syncwarp();
+                    float *rs = srs + lane, *ra = sra + lane;
+                    const float a0 = q.sx * rs[0 * 32], a1 = q.sy * rs[1 * 32], a2 = q.sz * rs[2 * 32];
+                    const float b0 = q.sx * rs[3 * 32], b1 = q.sy * rs[4 * 32], b2 = q.sz * rs[5 * 32];
+#pragma unroll
+                    for (int f = 0; f < 6; ++f) rs[f * 32] = 0.f;
+                    ra[0 * 32] += q.r00 * a0 + q.r01 * a1 + q.r02 * a2;
+                    ra[1 * 32] += q.r10 * a0 + q.r11 * a1 + q.r12 * a2;
+                    ra[2 * 32] += q.r20 * a0 + q.r21 * a1 + q.r22 * a2;
+                    ra[3 * 32] += q.r00 * b0 + q.r01 * b1 + q.r02 * b2;
+                    ra[4 * 32] += q.r10 * b0 + q.r11 * b1 + q.r12 * b2;
+                    ra[5 * 32] += q.r20 * b0 + q.r21 * b1 + q.r22 * b2;
+                    __syncwarp();
+                }
                 float g[16];
                 g[0] = q.r00 * gx[0] + q.r10 * gx[3] + q.r20 * gx[6];
                 g[1] = q.r01 * gx[1] + q.r11 * gx[4] + q.r21 * gx[7];
@@ -2491,12 +2574,19 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
             }   // while (word)
         }       // for (w)
     }           // for (cs)
+    if (kRayGrad) {
+        const float *ra = sra + lane;
+        store_ray_grads(p, n, tx, ty, lane, ra[0 * 32], ra[1 * 32], ra[2 * 32], ra[3 * 32], ra[4 * 32], ra[5 * 32],
+                        hashit ? L_TMIN : 0.f, rdx, rdy, rdz);
+    }
     return true;
 }
 
-template <int T, int CAP, bool kWarp, typename V>
+// kRayGrad: also write the per-ray gradients p.g_raypos / g_raydir / g_tminmax (mvp_raymarch_backward_rays); false compiles to
+// the plain backward
+template <int T, int CAP, bool kWarp, typename V, bool kRayGrad = false>
 __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_BWD_MINB * 4) / kWarps : 12 / kWarps) render_backward_kernel(const Params p) {
-    __shared__ BwdWarpSmem<CAP> s_w[kWarps];
+    __shared__ typename BwdSmemOf<CAP, kRayGrad>::type s_w[kWarps];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     BwdWarpSmem<CAP> *const S = &s_w[warp];
     if (CAP == kMaxHit) {
@@ -2504,7 +2594,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         for (int i = blockIdx.x * kWarps + warp; i < cnt; i += gridDim.x * kWarps) {
             const int id = p.heavylist[i];
             const int tx = id % p.TXn, ty = (id / p.TXn) % p.TYn, n = id / (p.TXn * p.TYn);
-            backward_tile<T, CAP, kWarp, V>(p, n, tx, ty, lane, S);
+            backward_tile<T, CAP, kWarp, V, kRayGrad>(p, n, tx, ty, lane, S);
             __syncwarp();
         }
     } else {
@@ -2517,7 +2607,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         const int tx = blockIdx.x * kBlkTX + (warp % kBlkTX), ty = blockIdx.y * kBlkTY + (warp / kBlkTX), n = blockIdx.z;
 #endif
         if (tx >= p.TXn || ty >= p.TYn) return;
-        if (!backward_tile<T, CAP, kWarp, V>(p, n, tx, ty, lane, S) && lane == 0)
+        if (!backward_tile<T, CAP, kWarp, V, kRayGrad>(p, n, tx, ty, lane, S) && lane == 0)
             p.heavylist[atomicAdd(p.heavycnt, 1)] = (n * p.TYn + ty) * p.TXn + tx;
     }
 }
@@ -2739,7 +2829,7 @@ const char *mvp_build_config(void) {
     return "LIST_REUSE=" MVP_STR(MVP_LIST_REUSE)
            " LIST_MARGIN=" MVP_STR(MVP_LIST_MARGIN) " XBUCKETS=" MVP_STR(MVP_XBUCKETS) " FASTCAP=" MVP_STR(MVP_FWD_FASTCAP) "/" MVP_STR(MVP_BWD_FASTCAP) " SMEM_UNION=" MVP_STR(MVP_SMEM_UNION) " CARVEOUT=" MVP_STR(MVP_FWD_CARVEOUT) "/" MVP_STR(MVP_BWD_CARVEOUT) " FWD_RING=" MVP_STR(MVP_FWD_RING) " BWD_SMEMREC=" MVP_STR(MVP_BWD_SMEMREC) " BWD_LANESMEM=" MVP_STR(MVP_BWD_LANESMEM) " CTA_ORDER=" MVP_STR(MVP_CTA_ORDER) " CTA_ORDER_MIN=" MVP_STR(MVP_CTA_ORDER_MIN)
            " CHUNK=" MVP_STR(MVP_CHUNK) " FWD_MINB=" MVP_STR(MVP_FWD_MINB) " BWD_MINB=" MVP_STR(MVP_BWD_MINB)
-           " WARPS=" MVP_STR(MVP_WARPS) " BLK_TX=" MVP_STR(MVP_BLK_TX) " TPLATE_BF16=1 EPILOGUE_BF16=1"
+           " WARPS=" MVP_STR(MVP_WARPS) " BLK_TX=" MVP_STR(MVP_BLK_TX) " TPLATE_BF16=1 EPILOGUE_BF16=1 RAY_GRADS=1"
 #ifdef MVP_CPU_EMUL
            " CPU_EMUL"
 #endif
@@ -2944,9 +3034,9 @@ int mvp_raymarch_forward(const mvp_forward_args *a, void *stream) {
     return e == cudaSuccess ? MVP_OK : (int)e;
 }
 
-int mvp_raymarch_backward(const mvp_backward_args *a, void *stream) {
-    if (!a) return MVP_ERR_NULL;
-    if (a->struct_size != sizeof(mvp_backward_args)) return MVP_ERR_STRUCT;
+// mvp_raymarch_backward, and with rays = true mvp_raymarch_backward_rays (grad_raypos / grad_raydir / grad_tminmax checked by the caller
+// for NULL; every other check is made here, before any device work)
+static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_raypos, float *grad_raydir, float *grad_tminmax, void *stream) {
     const int camrc = check_camera(a->camera);
     if (camrc < 0) return camrc;
     const mvp_camera *const camera = camrc ? &a->camera : nullptr;
@@ -2969,7 +3059,8 @@ int mvp_raymarch_backward(const mvp_backward_args *a, void *stream) {
         misaligned(a->tminmax, 8) || misaligned(a->raypos, 4) || misaligned(a->raydir, 4) || misaligned(a->primpos, 4) ||
         misaligned(a->primrot, 4) || misaligned(a->primscale, 4) || misaligned(a->raysat, 4) || misaligned(a->grad_primpos, 4) ||
         misaligned(a->grad_primrot, 4) || misaligned(a->grad_primscale, 4) || misaligned(a->warp, 4) || misaligned(a->grad_warp, 4) ||
-        misaligned(a->grad_rayrgb_nchw, 4) || misaligned(a->grad_rayalpha_nchw, 4) || misaligned(a->order, 4))
+        misaligned(a->grad_rayrgb_nchw, 4) || misaligned(a->grad_rayalpha_nchw, 4) || misaligned(a->order, 4) ||
+        misaligned(grad_raypos, 4) || misaligned(grad_raydir, 4) || misaligned(grad_tminmax, 8))
         return MVP_ERR_ALIGN;
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)a->workspace;
@@ -2999,6 +3090,7 @@ int mvp_raymarch_backward(const mvp_backward_args *a, void *stream) {
     p.grad_rayrgba = a->grad_rayrgba; p.raysat_in = a->raysat; p.rayaux_in = reinterpret_cast<const int4 *>(a->rayaux);
     p.g_primpos = a->grad_primpos; p.g_primrot = a->grad_primrot; p.g_primscale = a->grad_primscale; p.g_tplate = a->grad_tplate;
     p.warp = a->warp; p.g_warp = a->grad_warp; p.WD = a->WD; p.WH = a->WH; p.WW = a->WW;
+    p.g_raypos = grad_raypos; p.g_raydir = grad_raydir; p.g_tminmax = reinterpret_cast<float2 *>(grad_tminmax);
 #if MVP_CTA_ORDER
     dim3 grid((unsigned)((size_t)p.CXn * p.CYn * a->shape.N));
 #else
@@ -3012,11 +3104,17 @@ int mvp_raymarch_backward(const mvp_backward_args *a, void *stream) {
     const int cubic = (a->shape.TD == a->shape.TH && a->shape.TH == a->shape.TW) ? a->shape.TD : 0;
     int heavy = 0;
     if (int eh = heavy_grid(&heavy)) return eh;
-#define MVP_LAUNCH_BWD(TT, WW_, VV)                                                              \
-    do {                                                                                         \
-        MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV>);             \
-        MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV>);                         \
-        MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV>);                          \
+#define MVP_LAUNCH_BWD(TT, WW_, VV)                                                                          \
+    do {                                                                                                     \
+        if (rays) {                                                                                          \
+            MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV, true>);               \
+            MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV, true>);                           \
+            MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV, true>);                            \
+        } else {                                                                                             \
+            MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV>);                     \
+            MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV>);                                 \
+            MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV>);                                  \
+        }                                                                                                    \
     } while (0)
 #define MVP_LAUNCH_BWD_T(VV)                                                                     \
     do {                                                                                         \
@@ -3031,6 +3129,19 @@ int mvp_raymarch_backward(const mvp_backward_args *a, void *stream) {
 #undef MVP_LAUNCH_BWD
     cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? MVP_OK : (int)e;
+}
+
+int mvp_raymarch_backward(const mvp_backward_args *a, void *stream) {
+    if (!a) return MVP_ERR_NULL;
+    if (a->struct_size != sizeof(mvp_backward_args)) return MVP_ERR_STRUCT;
+    return backward_impl(a, false, nullptr, nullptr, nullptr, stream);
+}
+
+int mvp_raymarch_backward_rays(const mvp_backward_args *a, float *grad_raypos, float *grad_raydir, float *grad_tminmax, void *stream) {
+    if (!a) return MVP_ERR_NULL;
+    if (a->struct_size != sizeof(mvp_backward_args)) return MVP_ERR_STRUCT;
+    if (!grad_raypos || !grad_raydir || !grad_tminmax) return MVP_ERR_NULL;
+    return backward_impl(a, true, grad_raypos, grad_raydir, grad_tminmax, stream);
 }
 
 #if defined(MVP_CPU_EMUL) && defined(MVP_EMUL_STATS)

@@ -84,7 +84,7 @@ EXPORTS = ("mvp_abi_version", "mvp_build_config", "mvp_error_string", "mvp_works
            "mvp_assemble_payload_backward", "mvp_debug_saved_tiles", "mvp_debug_tileclk_offset", "mvp_debug_heavy_offset",
            "mvp_compute_morton",
            "mvp_expand_views", "mvp_sum_views", "mvp_assemble_payload_forward_bf16", "mvp_assemble_payload_backward_bf16",
-           "mvp_sum_views_bf16")
+           "mvp_sum_views_bf16", "mvp_raymarch_backward_rays", "mvp_compute_raydirs_backward")
 
 
 def _load():
@@ -121,6 +121,10 @@ def _load():
     lib.mvp_raymarch_backward.argtypes = [ctypes.POINTER(BackwardArgs), c_f]
     lib.mvp_compute_raydirs.restype = ctypes.c_int
     lib.mvp_compute_raydirs.argtypes = [ctypes.c_int32] * 3 + [c_f] * 5 + [ctypes.c_float] + [c_f] * 4
+    lib.mvp_raymarch_backward_rays.restype = ctypes.c_int
+    lib.mvp_raymarch_backward_rays.argtypes = [ctypes.POINTER(BackwardArgs)] + [c_f] * 4
+    lib.mvp_compute_raydirs_backward.restype = ctypes.c_int
+    lib.mvp_compute_raydirs_backward.argtypes = [ctypes.c_int32] * 3 + [c_f] * 5 + [ctypes.c_float] + [c_f] * 8
     lib.mvp_composite_forward.restype = ctypes.c_int
     lib.mvp_composite_forward.argtypes = [ctypes.c_int32] * 3 + [c_f] * 7
     lib.mvp_composite_backward.restype = ctypes.c_int
@@ -176,6 +180,13 @@ def require_epilogue_bf16():
     which it reports as EPILOGUE_BF16=1 in its build configuration."""
     if "EPILOGUE_BF16=1" not in LIB.mvp_build_config().decode().split():
         raise RuntimeError("mvpraymarch_b200: this library (%s) does not support bfloat16 payload hand-off" % _build.LIB)
+
+
+def require_ray_grads():
+    """Raise unless the library has the ray-gradient backward and the ray generator's adjoint (mvp_raymarch_backward_rays,
+    mvp_compute_raydirs_backward), which it reports as RAY_GRADS=1 in its build configuration."""
+    if "RAY_GRADS=1" not in LIB.mvp_build_config().decode().split():
+        raise RuntimeError("mvpraymarch_b200: this library (%s) does not support gradients of rays and cameras" % _build.LIB)
 
 
 def workspace_bytes(N, H, W, K, TD, TH, TW):

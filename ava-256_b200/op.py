@@ -57,6 +57,13 @@ class MVPRaymarch(Function):
     @staticmethod
     def forward(ctx, raypos, raydir, stepsize, tminmax, primpos, primrot, primscale, template, warp, rayterm,
                 gradmode, options):
+        return MVPRaymarch._forward(ctx, raypos, raydir, stepsize, tminmax, primpos, primrot, primscale, template, warp, rayterm,
+                                    gradmode, options)
+
+    @staticmethod
+    def _forward(ctx, raypos, raydir, stepsize, tminmax, primpos, primrot, primscale, template, warp, rayterm,
+                 gradmode, options, saved_extra=()):
+        """The forward; saved_extra: more tensors for ctx.save_for_backward, after the eleven the backward reads."""
         algo = options["algo"]
         if algo not in (0, 1):
             raise NotImplementedError("mvpraymarch_b200: algo must be 0 or 1 (the reference launches nothing for other "
@@ -168,8 +175,9 @@ class MVPRaymarch(Function):
 
         if gradmode:
             ctx.grads = grads
-            ctx.save_for_backward(raypos, raydir, tminmax, primpos, primrot, primscale, template, raysat, rayaux, workspace, warp)
-            ctx.camera = camera                # camera tensors are plain inputs without gradients (utils.py:45-46 returns None for all)
+            ctx.save_for_backward(raypos, raydir, tminmax, primpos, primrot, primscale, template, raysat, rayaux, workspace, warp,
+                                  *saved_extra)
+            ctx.camera = camera                # camera tensors: no gradients (utils.py:45-46), except through MVPRaymarchCameraGrad
             ctx.nhw = (N, H, W)
             ctx.order = order
             ctx.options = options
@@ -182,56 +190,73 @@ class MVPRaymarch(Function):
 
     @staticmethod
     def backward(ctx, grad_rayrgba, grad_rayalpha=None):
-        """grad_rayrgba [N,H,W,4]; or, for MVPRaymarchPlanes, (grad_rayrgb [N,3,H,W], grad_rayalpha [N,1,H,W])."""
-        raypos, raydir, tminmax, primpos, primrot, primscale, template, raysat, rayaux, workspace, warp = ctx.saved_tensors
-        options = ctx.options
-        N, H, W = ctx.nhw
-        K = primpos.size(1)
-        TD, TH, TW = template.shape[2:5]
-        dev = primpos.device
-        with torch.cuda.device(dev):
-            planes = bool(options.get("_planes", False))
-            if planes:
-                grad_rgb = grad_rayrgba.contiguous() if grad_rayrgba is not None else torch.zeros((N, 3, H, W), device=dev)
-                grad_alpha = grad_rayalpha.contiguous() if grad_rayalpha is not None else torch.zeros((N, 1, H, W), device=dev)
-                grad_rayrgba = None
-            else:
-                grad_rayrgba = _aligned(grad_rayrgba.contiguous(), 16)     # mvpraymarch.py:264
-            usewarp = options["algo"] == 1
-            grads, ctx.grads = ctx.grads, None
-            fresh = grads is not None          # the forward's render kernel zero-filled them; a second backward through the
-            if not fresh:                      # same graph (retain_graph) gets new ones, zero-filled by the library
-                grads = [torch.empty_like(primpos), torch.empty_like(primrot), torch.empty_like(primscale), torch.empty_like(template),
-                         torch.empty_like(warp) if usewarp else None]
-            grad_primpos, grad_primrot, grad_primscale, grad_template, grad_warp = grads
-            if warp is not None and not usewarp:                       # mvpraymarch.py:246 (zero when algo 0 ignores it)
-                grad_warp = torch.zeros_like(warp)
-            a = _lib.BackwardArgs()
-            a.shape = _lib.Shape(N, H, W, K, TD, TH, TW)
-            a.stepsize, a.fadescale, a.fadeexp = ctx.stepsize, float(options["fadescale"]), float(options["fadeexp"])
-            a.flags = _lib.FLAG_ACCEL_VALID | (0 if fresh else _lib.FLAG_ZERO_GRADS) | (_lib.FLAG_SHARED_PRIMS if ctx.shared else 0) | \
-                ctx.tflags
-            a.raypos, a.raydir, a.tminmax = _ptr(raypos), _ptr(raydir), _ptr(tminmax)
-            if ctx.camera is not None:
-                viewpos, viewrot, focal, princpt, volradius = ctx.camera[:5]
-                a.camera = _lib.Camera(_ptr(viewpos), _ptr(viewrot), _ptr(focal), _ptr(princpt), float(volradius), 0)
-            a.primpos, a.primrot, a.primscale = _ptr(primpos), _ptr(primrot), _ptr(primscale)
-            a.tplate = _ptr(template)
-            a.grad_rayrgba, a.raysat, a.rayaux = _ptr(grad_rayrgba), _ptr(raysat), _ptr(rayaux)
-            if planes:
-                a.grad_rayrgb_nchw, a.grad_rayalpha_nchw = _ptr(grad_rgb), _ptr(grad_alpha)
-            if ctx.order is not None:
-                a.order = _ptr(ctx.order)
-            a.grad_primpos, a.grad_primrot, a.grad_primscale = _ptr(grad_primpos), _ptr(grad_primrot), _ptr(grad_primscale)
-            a.grad_tplate = _ptr(grad_template)
-            a.workspace, a.workspace_bytes = _ptr(workspace), workspace.numel()
-            a.algo = 1 if usewarp else 0
-            if usewarp:
-                a.warp, a.grad_warp = _ptr(warp), _ptr(grad_warp)
-                a.WD, a.WH, a.WW = warp.shape[2:5]
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            _lib.check(_lib.LIB.mvp_raymarch_backward(ctypes.byref(a), ctypes.c_void_p(stream)))
-        return (None, None, None, None, grad_primpos, grad_primrot, grad_primscale, grad_template, grad_warp, None, None, None)
+        """grad_rayrgba [N,H,W,4]; or, for MVPRaymarchPlanes, (grad_rayrgb [N,3,H,W], grad_rayalpha [N,1,H,W]).  With the
+        `_ray_grads` option (a differentiable `compute_raydirs` feeds the rays, see `mvpraymarch_camera`) the rays get gradients too."""
+        want_rays = bool(ctx.options.get("_ray_grads")) and any(ctx.needs_input_grad[i] for i in (0, 1, 3))
+        prim, rays = _march_backward(ctx, grad_rayrgba, grad_rayalpha, want_rays)
+        grad_raypos, grad_raydir, grad_tminmax = rays if rays is not None else (None, None, None)
+        return (grad_raypos, grad_raydir, None, grad_tminmax) + prim + (None, None, None)
+
+
+def _march_backward(ctx, grad_rayrgba, grad_rayalpha, want_rays):
+    """The native backward of an MVPRaymarch forward: ((grad_primpos, grad_primrot, grad_primscale, grad_template, grad_warp),
+    (grad_raypos, grad_raydir, grad_tminmax) with want_rays (mvp_raymarch_backward_rays), else None)."""
+    raypos, raydir, tminmax, primpos, primrot, primscale, template, raysat, rayaux, workspace, warp = ctx.saved_tensors[:11]
+    options = ctx.options
+    N, H, W = ctx.nhw
+    K = primpos.size(1)
+    TD, TH, TW = template.shape[2:5]
+    dev = primpos.device
+    with torch.cuda.device(dev):
+        planes = bool(options.get("_planes", False))
+        if planes:
+            grad_rgb = grad_rayrgba.contiguous() if grad_rayrgba is not None else torch.zeros((N, 3, H, W), device=dev)
+            grad_alpha = grad_rayalpha.contiguous() if grad_rayalpha is not None else torch.zeros((N, 1, H, W), device=dev)
+            grad_rayrgba = None
+        else:
+            grad_rayrgba = _aligned(grad_rayrgba.contiguous(), 16)     # mvpraymarch.py:264
+        usewarp = options["algo"] == 1
+        grads, ctx.grads = ctx.grads, None
+        fresh = grads is not None          # the forward's render kernel zero-filled them; a second backward through the
+        if not fresh:                      # same graph (retain_graph) gets new ones, zero-filled by the library
+            grads = [torch.empty_like(primpos), torch.empty_like(primrot), torch.empty_like(primscale), torch.empty_like(template),
+                     torch.empty_like(warp) if usewarp else None]
+        grad_primpos, grad_primrot, grad_primscale, grad_template, grad_warp = grads
+        if warp is not None and not usewarp:                       # mvpraymarch.py:246 (zero when algo 0 ignores it)
+            grad_warp = torch.zeros_like(warp)
+        a = _lib.BackwardArgs()
+        a.shape = _lib.Shape(N, H, W, K, TD, TH, TW)
+        a.stepsize, a.fadescale, a.fadeexp = ctx.stepsize, float(options["fadescale"]), float(options["fadeexp"])
+        a.flags = _lib.FLAG_ACCEL_VALID | (0 if fresh else _lib.FLAG_ZERO_GRADS) | (_lib.FLAG_SHARED_PRIMS if ctx.shared else 0) | \
+            ctx.tflags
+        a.raypos, a.raydir, a.tminmax = _ptr(raypos), _ptr(raydir), _ptr(tminmax)
+        if ctx.camera is not None:
+            viewpos, viewrot, focal, princpt, volradius = ctx.camera[:5]
+            a.camera = _lib.Camera(_ptr(viewpos), _ptr(viewrot), _ptr(focal), _ptr(princpt), float(volradius), 0)
+        a.primpos, a.primrot, a.primscale = _ptr(primpos), _ptr(primrot), _ptr(primscale)
+        a.tplate = _ptr(template)
+        a.grad_rayrgba, a.raysat, a.rayaux = _ptr(grad_rayrgba), _ptr(raysat), _ptr(rayaux)
+        if planes:
+            a.grad_rayrgb_nchw, a.grad_rayalpha_nchw = _ptr(grad_rgb), _ptr(grad_alpha)
+        if ctx.order is not None:
+            a.order = _ptr(ctx.order)
+        a.grad_primpos, a.grad_primrot, a.grad_primscale = _ptr(grad_primpos), _ptr(grad_primrot), _ptr(grad_primscale)
+        a.grad_tplate = _ptr(grad_template)
+        a.workspace, a.workspace_bytes = _ptr(workspace), workspace.numel()
+        a.algo = 1 if usewarp else 0
+        if usewarp:
+            a.warp, a.grad_warp = _ptr(warp), _ptr(grad_warp)
+            a.WD, a.WH, a.WW = warp.shape[2:5]
+        stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        rays = None
+        if want_rays:
+            _lib.require_ray_grads()
+            # written for every ray by the library: no zero-fill
+            rays = (torch.empty((N, H, W, 3), device=dev), torch.empty((N, H, W, 3), device=dev), torch.empty((N, H, W, 2), device=dev))
+            _lib.check(_lib.LIB.mvp_raymarch_backward_rays(ctypes.byref(a), *(_ptr(t) for t in rays), stream))
+        else:
+            _lib.check(_lib.LIB.mvp_raymarch_backward(ctypes.byref(a), stream))
+    return (grad_primpos, grad_primrot, grad_primscale, grad_template, grad_warp), rays
 
 
 class MVPRaymarchPlanes(MVPRaymarch):
@@ -249,6 +274,28 @@ class MVPRaymarchPlanes(MVPRaymarch):
     @staticmethod
     def backward(ctx, grad_rayrgb, grad_rayalpha):
         return MVPRaymarch.backward(ctx, grad_rayrgb, grad_rayalpha)
+
+
+class MVPRaymarchCameraGrad(Function):
+    """The camera form of the op (`options["_camera"]`: rays generated in the kernels) with the four camera tensors as autograd
+    inputs: the backward writes each ray's gradient into a temporary 32 B/ray buffer (mvp_raymarch_backward_rays) and the ray
+    generator's adjoint (mvp_compute_raydirs_backward) reduces them per view.  Outputs as MVPRaymarch (or its planes form)."""
+
+    @staticmethod
+    def forward(ctx, viewpos, viewrot, focal, princpt, stepsize, primpos, primrot, primscale, template, warp, gradmode, options):
+        # the camera tensors are saved for backward: the adjoint recomputes the rays from them
+        return MVPRaymarch._forward(ctx, None, None, stepsize, None, primpos, primrot, primscale, template, warp, None, gradmode, options,
+                                    saved_extra=(viewpos, viewrot, focal, princpt))
+
+    @staticmethod
+    def backward(ctx, grad_out, grad_rayalpha=None):
+        prim, rays = _march_backward(ctx, grad_out, grad_rayalpha, True)
+        viewpos, viewrot, focal, princpt = ctx.saved_tensors[11:15]
+        volradius = ctx.camera[4]
+        from .raydirs import raydirs_backward
+        cam = raydirs_backward(viewpos, viewrot, focal, princpt, None, volradius, *rays)
+        cam = tuple(g if need else None for g, need in zip(cam, ctx.needs_input_grad[:4]))
+        return cam + (None,) + prim + (None, None)
 
 
 def morton_codes(primpos):
@@ -358,13 +405,21 @@ def mvpraymarch(
     }
     if _CAMERA.get("cam") is not None:
         options["_camera"] = _CAMERA["cam"]
+    if _CAMERA.get("grad"):
+        options["_ray_grads"] = True
+        if options.get("_camera") is not None:
+            if _PLANES.get("on"):
+                options["_planes"] = True
+            viewpos, viewrot, focal, princpt = options["_camera"][:4]
+            return MVPRaymarchCameraGrad.apply(viewpos, viewrot, focal, princpt, stepsize, primpos, primrot, primscale, template, warp,
+                                               torch.is_grad_enabled(), options)
     fn = MVPRaymarchPlanes if _PLANES.get("on") else MVPRaymarch
     return fn.apply(raypos, raydir, stepsize, tminmax, primpos, primrot, primscale, template, warp, rayterm,
                     torch.is_grad_enabled(), options)
 
 
 _PLANES = {}
-_CAMERA = {}
+_CAMERA = {}     # "cam": the camera of a mvpraymarch_camera call (rays generated in the kernels); "grad": camera_grad=True
 
 
 def mvpraymarch_planes(*args, **kwargs):
@@ -378,7 +433,7 @@ def mvpraymarch_planes(*args, **kwargs):
 
 
 def mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, volradius, stepsize, primtransf, template, warp, planes=False,
-                       **kwargs):
+                       camera_grad=False, **kwargs):
     """`compute_raydirs` + `mvpraymarch` of models/autoencoder.py:240-252 as ONE call: the first six parameters are those of the
     reference's compute_raydirs (extensions/utils/utils.py:48-51), the rest those of `mvpraymarch` after its ray arguments.
 
@@ -387,16 +442,29 @@ def mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, volradius,
     `compute_raydirs` would have written -- 32 bytes per ray that are neither written by a generation pass nor read by forward
     and backward -- and the accel build takes the camera as it is instead of fitting one to the ray field.  With a `pixelcoords`
     tensor (arbitrary sample positions) the two calls are made one after the other, as in the reference.
-    No gradients flow to the camera (the reference's compute_raydirs backward returns None for every input, utils.py:45-46).
+    By default no gradients flow to the camera, like the reference (its compute_raydirs backward returns None for every input,
+    utils.py:45-46).  With camera_grad=True, viewpos, viewrot, focal and princpt are autograd inputs and those that require grad get
+    the gradient of the image with every discrete decision of the march held fixed (C-ABI mvp_raymarch_backward_rays, then the ray
+    generator's adjoint mvp_compute_raydirs_backward); pixelcoords and volradius get none.  When no camera tensor requires grad,
+    the plain backward runs.
     Returns rayrgba [N,H,W,4], or (rayrgb [N,3,H,W], rayalpha [N,1,H,W]) with planes=True."""
     march = mvpraymarch_planes if planes else mvpraymarch
+    grad = bool(camera_grad) and torch.is_grad_enabled() and any(t.requires_grad for t in (viewpos, viewrot, focal, princpt))
+    if grad:
+        _lib.require_ray_grads()
     if not isinstance(pixelcoords, tuple):
         from .raydirs import compute_raydirs
-        raypos, raydir, tminmax = compute_raydirs(viewpos, viewrot, focal, princpt, pixelcoords, volradius)
-        return march(raypos, raydir, stepsize, tminmax, primtransf, template, warp, **kwargs)
+        raypos, raydir, tminmax = compute_raydirs(viewpos, viewrot, focal, princpt, pixelcoords, volradius, differentiable=grad)
+        _CAMERA["grad"] = grad
+        try:
+            return march(raypos, raydir, stepsize, tminmax, primtransf, template, warp, **kwargs)
+        finally:
+            _CAMERA["grad"] = False
     W, H = pixelcoords
     _CAMERA["cam"] = (viewpos, viewrot, focal, princpt, float(volradius), int(H), int(W))
+    _CAMERA["grad"] = grad
     try:
         return march(None, None, stepsize, None, primtransf, template, warp, **kwargs)
     finally:
         _CAMERA["cam"] = None
+        _CAMERA["grad"] = False

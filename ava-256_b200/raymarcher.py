@@ -29,14 +29,16 @@ class Raymarcher(nn.Module):
         rayrgb, rayalpha = mvpraymarch_planes(*args, **kwargs)
         return rayrgb, rayalpha, None, None
 
-    def forward_camera(self, viewpos, viewrot, focal, princpt, pixelcoords, decout, renderoptions={}, rayterm=None):
+    def forward_camera(self, viewpos, viewrot, focal, princpt, pixelcoords, decout, renderoptions={}, rayterm=None, camera_grad=False):
         """`compute_raydirs(viewpos, viewrot, focal, princpt, pixelcoords, volradius)` followed by `forward(raypos, raydir, tminmax,
         ...)` -- models/autoencoder.py:240-252 -- as one call.  With `pixelcoords = (W, H)` the rays are generated inside the render
-        kernels and never stored (`op.mvpraymarch_camera`); same return tuple as `forward`."""
+        kernels and never stored (`op.mvpraymarch_camera`); same return tuple as `forward`.  camera_grad=True: the camera tensors
+        that require grad get gradients (pose / calibration fitting through the image loss, see `op.mvpraymarch_camera`)."""
         kwargs = dict(rayterm=rayterm, **{k: v for k, v in renderoptions.items() if k in mvpraymarch.__code__.co_varnames})
         out = mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, self.volume_radius, self.dt,
                                  (decout["primpos"], decout["primrot"], decout["primscale"]), decout["template"],
-                                 decout["warp"] if "warp" in decout else None, planes=not self.with_rgba, **kwargs)
+                                 decout["warp"] if "warp" in decout else None, planes=not self.with_rgba, camera_grad=camera_grad,
+                                 **kwargs)
         if self.with_rgba:
             rayrgb, rayalpha = split_rgba(out)
             return rayrgb, rayalpha, out.permute(0, 3, 1, 2), None

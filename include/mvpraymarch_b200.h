@@ -193,6 +193,17 @@ int mvp_compute_morton(int32_t N, int32_t K, const float *centre, int32_t *code,
 
 int mvp_raymarch_forward(const mvp_forward_args *args, void *stream);
 int mvp_raymarch_backward(const mvp_backward_args *args, void *stream);
+/* mvp_raymarch_backward plus the gradients of the rays, in the ray-tensor and in the camera form (args->camera): everything
+ * mvp_raymarch_backward does, and grad_raypos, grad_raydir [N,H,W,3] and grad_tminmax [N,H,W,2] are WRITTEN (not accumulated),
+ * one value per ray, rays that take no sample included.  The gradient is that of the image with every discrete decision of the
+ * march held fixed (candidate lists, first lattice step, the strict validity test, the saturating sample, the 512-entry cap):
+ * with the ray's samples x_j = raypos + raydir (tmin + j stepsize) up to and including the saturating one,
+ *   grad_raypos = sum_j dL/dx_j,   grad_raydir = sum_j (tmin + j stepsize) dL/dx_j,   grad_tminmax = (<raydir, grad_raypos>, 0),
+ * which is what autograd gives for the reference's PyTorch loop (extensions/mvpraymarch/mvpraymarch.py:567-633) with its sample
+ * positions left attached.  grad_raypos / grad_raydir 4-byte aligned, grad_tminmax 8;
+ * argument errors are returned before any device work.  The library supports it iff mvp_build_config() lists RAY_GRADS=1. */
+int mvp_raymarch_backward_rays(const mvp_backward_args *args, float *grad_raypos, float *grad_raydir, float *grad_tminmax,
+                               void *stream);
 
 /* Pinhole ray generation + unit-cube clip (reference: extensions/utils/utils_kernel.cu:12-52).
  * viewpos [N,3], viewrot [N,3,3], focal [N,2], princpt [N,2], pixelcoords [N,H,W,2] or NULL (integer grid);
@@ -200,6 +211,17 @@ int mvp_raymarch_backward(const mvp_backward_args *args, void *stream);
 int mvp_compute_raydirs(int32_t N, int32_t H, int32_t W, const float *viewpos, const float *viewrot, const float *focal,
                         const float *princpt, const float *pixelcoords, float volradius, float *raypos, float *raydir,
                         float *tminmax, void *stream);
+/* Adjoint of mvp_compute_raydirs (and of the rays an mvp_camera call generates): the per-ray gradients grad_raypos, grad_raydir
+ * [N,H,W,3] and grad_tminmax [N,H,W,2] (8-byte aligned, like pixelcoords) are chained through o = viewpos / volradius, the
+ * unit-cube clip of tmin (the face the forward's min/max chain selects; zero where tmin is clamped to 0; tmax has no gradient),
+ * d = e / |e|, e = viewrot^T (u, v, 1) and u = (px - princpt.x) / focal.x, v = (py - princpt.y) / focal.y into grad_viewpos [N,3],
+ * grad_viewrot [N,3,3], grad_focal [N,2] and grad_princpt [N,2], which are ACCUMULATED into: the caller zero-fills them.  Nothing
+ * goes to pixelcoords or volradius.  One thread per ray; the 16 per-view sums are reduced per block and added with one atomic per
+ * block and value, so the result is deterministic up to the order of those atomics. */
+int mvp_compute_raydirs_backward(int32_t N, int32_t H, int32_t W, const float *viewpos, const float *viewrot, const float *focal,
+                                 const float *princpt, const float *pixelcoords, float volradius, const float *grad_raypos,
+                                 const float *grad_raydir, const float *grad_tminmax, float *grad_viewpos, float *grad_viewrot,
+                                 float *grad_focal, float *grad_princpt, void *stream);
 
 /* Image epilogue (SURVEY.md section 8f row 2).  rayrgba [N,H,W,4] (16-byte aligned) ->
  *   irgbrec  [N,3,H,W] = (ccw[n,c] * rgb + ccb[n,c]) + (1 - alpha) * bg[n,c,h,w]      (each op rounded once, like eager torch)
