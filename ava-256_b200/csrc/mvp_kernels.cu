@@ -1394,6 +1394,14 @@ template <> struct Payload<Bf16x4> {
 #endif
     }
 };
+// A bf16 template whose gradient is accumulated in fp32 (MVP_FLAG_TPLATE_BF16 | MVP_FLAG_GRAD_TPLATE_F32): read like Bf16x4, the
+// gradient laid out and reduced like float4's, so it is the fp32 kernels' gradient on the widened template up to atomic order.
+struct __align__(8) Bf16x4G32 { unsigned lo, hi; };
+template <> struct Payload<Bf16x4G32> {
+    static constexpr unsigned kBytes = 8, kWords = 4;
+    static __device__ __forceinline__ float4 load(const Bf16x4G32 *v) { return Payload<Bf16x4>::load(reinterpret_cast<const Bf16x4 *>(v)); }
+    static __device__ __forceinline__ void red(float *g, size_t i, float a, float b, float c, float d) { red_add_v4(g + i * 4, a, b, c, d); }
+};
 
 // primsampler.h:44-66 + utils.h:408-502.  T > 0: cubic slab with compile-time strides; T == 0: runtime dims.
 // Only called for valid samples (|y| < 1), for which (a) the reference's +-100 clamp is a no-op and (b) the only
@@ -2829,7 +2837,7 @@ const char *mvp_build_config(void) {
     return "LIST_REUSE=" MVP_STR(MVP_LIST_REUSE)
            " LIST_MARGIN=" MVP_STR(MVP_LIST_MARGIN) " XBUCKETS=" MVP_STR(MVP_XBUCKETS) " FASTCAP=" MVP_STR(MVP_FWD_FASTCAP) "/" MVP_STR(MVP_BWD_FASTCAP) " SMEM_UNION=" MVP_STR(MVP_SMEM_UNION) " CARVEOUT=" MVP_STR(MVP_FWD_CARVEOUT) "/" MVP_STR(MVP_BWD_CARVEOUT) " FWD_RING=" MVP_STR(MVP_FWD_RING) " BWD_SMEMREC=" MVP_STR(MVP_BWD_SMEMREC) " BWD_LANESMEM=" MVP_STR(MVP_BWD_LANESMEM) " CTA_ORDER=" MVP_STR(MVP_CTA_ORDER) " CTA_ORDER_MIN=" MVP_STR(MVP_CTA_ORDER_MIN)
            " CHUNK=" MVP_STR(MVP_CHUNK) " FWD_MINB=" MVP_STR(MVP_FWD_MINB) " BWD_MINB=" MVP_STR(MVP_BWD_MINB)
-           " WARPS=" MVP_STR(MVP_WARPS) " BLK_TX=" MVP_STR(MVP_BLK_TX) " TPLATE_BF16=1 EPILOGUE_BF16=1 RAY_GRADS=1"
+           " WARPS=" MVP_STR(MVP_WARPS) " BLK_TX=" MVP_STR(MVP_BLK_TX) " TPLATE_BF16=1 EPILOGUE_BF16=1 RAY_GRADS=1 GRAD_TPLATE_F32=1"
 #ifdef MVP_CPU_EMUL
            " CPU_EMUL"
 #endif
@@ -2844,7 +2852,7 @@ const char *mvp_error_string(int code) {
         case MVP_ERR_STEPSIZE: return "stepsize must be finite and > 0";
         case MVP_ERR_WORKSPACE: return "workspace too small or not 256-byte aligned";
         case MVP_ERR_ALGO: return "unsupported algo";
-        case MVP_ERR_ALIGN: return "misaligned buffer (tplate/grad_tplate: 16 bytes, 8 with MVP_FLAG_TPLATE_BF16; rayrgba/grad_rayrgba/rayaux/clear_grad_*: 16, tminmax: 8, others: 4)";
+        case MVP_ERR_ALIGN: return "misaligned buffer (tplate/grad_tplate: 16 bytes, 8 with MVP_FLAG_TPLATE_BF16 (grad_tplate 16 with MVP_FLAG_GRAD_TPLATE_F32); rayrgba/grad_rayrgba/rayaux/clear_grad_*: 16, tminmax: 8, others: 4)";
         case MVP_ERR_STRUCT: return "args->struct_size does not match this library's argument struct (ABI mismatch)";
         case MVP_ERR_CAMERA: return "camera.volradius must be finite and > 0";
         default: return code > 0 ? cudaGetErrorString((cudaError_t)code) : "unknown error";
@@ -2921,6 +2929,11 @@ int mvp_backward_launch_count(uint32_t flags) { return (flags & MVP_FLAG_ACCEL_V
 
 static inline bool misaligned(const void *p, uintptr_t a) { return p && ((uintptr_t)p & (a - 1)); }
 
+// 4-byte words per voxel of the template gradient: bf16 (2) only for a bf16 template without MVP_FLAG_GRAD_TPLATE_F32
+static inline unsigned grad_tplate_words(uint32_t flags) {
+    return ((flags & MVP_FLAG_TPLATE_BF16) && !(flags & MVP_FLAG_GRAD_TPLATE_F32)) ? Payload<Bf16x4>::kWords : Payload<float4>::kWords;
+}
+
 int mvp_raymarch_forward(const mvp_forward_args *a, void *stream) {
     if (!a) return MVP_ERR_NULL;
     if (a->struct_size != sizeof(mvp_forward_args)) return MVP_ERR_STRUCT;
@@ -2985,7 +2998,7 @@ int mvp_raymarch_forward(const mvp_forward_args *a, void *stream) {
         float *const bufs[kClearBufs] = {a->clear_grad_primpos, a->clear_grad_primrot, a->clear_grad_primscale, a->clear_grad_tplate,
                                          a->algo == 1 ? a->clear_grad_warp : nullptr};
         // sizes in 4-byte words: a bf16 template gradient holds two channels per word
-        const size_t floats[kClearBufs] = {nk * 3, nk * 9, nk * 3, nk * a->shape.TD * a->shape.TH * a->shape.TW * (bf16 ? 2 : 4),
+        const size_t floats[kClearBufs] = {nk * 3, nk * 9, nk * 3, nk * a->shape.TD * a->shape.TH * a->shape.TW * grad_tplate_words(a->flags),
                                            a->algo == 1 ? nk * a->WD * a->WH * a->WW * 3 : 0};
         for (int b = 0; b < kClearBufs; ++b) {
             if (!bufs[b]) continue;
@@ -3055,7 +3068,8 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
     const Layout L = make_layout(a->shape);
     if (a->workspace_bytes < L.total || ((uintptr_t)a->workspace & 255)) return MVP_ERR_WORKSPACE;
     const bool bf16 = (a->flags & MVP_FLAG_TPLATE_BF16) != 0;
-    if (misaligned(a->tplate, bf16 ? 8 : 16) || misaligned(a->grad_tplate, bf16 ? 8 : 16) || misaligned(a->grad_rayrgba, 16) || misaligned(a->rayaux, 16) ||
+    const unsigned gwords = grad_tplate_words(a->flags);
+    if (misaligned(a->tplate, bf16 ? 8 : 16) || misaligned(a->grad_tplate, gwords * 4) || misaligned(a->grad_rayrgba, 16) || misaligned(a->rayaux, 16) ||
         misaligned(a->tminmax, 8) || misaligned(a->raypos, 4) || misaligned(a->raydir, 4) || misaligned(a->primpos, 4) ||
         misaligned(a->primrot, 4) || misaligned(a->primscale, 4) || misaligned(a->raysat, 4) || misaligned(a->grad_primpos, 4) ||
         misaligned(a->grad_primrot, 4) || misaligned(a->grad_primscale, 4) || misaligned(a->warp, 4) || misaligned(a->grad_warp, 4) ||
@@ -3075,7 +3089,7 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
         if (z == cudaSuccess) z = cudaMemsetAsync(a->grad_primrot, 0, nk * 9 * sizeof(float), st);
         if (z == cudaSuccess) z = cudaMemsetAsync(a->grad_primscale, 0, nk * 3 * sizeof(float), st);
         if (z == cudaSuccess)
-            z = cudaMemsetAsync(a->grad_tplate, 0, nk * a->shape.TD * a->shape.TH * a->shape.TW * (bf16 ? Payload<Bf16x4>::kBytes : Payload<float4>::kBytes), st);
+            z = cudaMemsetAsync(a->grad_tplate, 0, nk * a->shape.TD * a->shape.TH * a->shape.TW * gwords * sizeof(float), st);
         if (z == cudaSuccess && a->algo == 1) z = cudaMemsetAsync(a->grad_warp, 0, nk * a->WD * a->WH * a->WW * 3 * sizeof(float), st);
         if (z != cudaSuccess) return (int)z;
     }
@@ -3123,7 +3137,8 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
         else if (cubic == 16) MVP_LAUNCH_BWD(16, false, VV);                                     \
         else MVP_LAUNCH_BWD(0, false, VV);                                                       \
     } while (0)
-    if (bf16) MVP_LAUNCH_BWD_T(Bf16x4);
+    if (bf16 && gwords == Payload<Bf16x4G32>::kWords) MVP_LAUNCH_BWD_T(Bf16x4G32);
+    else if (bf16) MVP_LAUNCH_BWD_T(Bf16x4);
     else MVP_LAUNCH_BWD_T(float4);
 #undef MVP_LAUNCH_BWD_T
 #undef MVP_LAUNCH_BWD

@@ -72,6 +72,7 @@ FLAG_ACCEL_VALID = 1
 FLAG_ZERO_GRADS = 2
 FLAG_SHARED_PRIMS = 4
 FLAG_TPLATE_BF16 = 8
+FLAG_GRAD_TPLATE_F32 = 16
 FLAG_TEST_TINY_LISTS = 0x100
 ABI_VERSION = 8
 # layout pins, equal to the static_asserts in csrc/mvp_kernels.cu (tests/test_abi.py compares)
@@ -164,15 +165,22 @@ def check(rc):
         raise RuntimeError("mvpraymarch_b200: %s (code %d)" % (LIB.mvp_error_string(rc).decode(), rc))
 
 
-def tplate_flags(bf16):
-    """The flag bits that tell the raymarch calls the template's dtype: MVP_FLAG_TPLATE_BF16 for a bfloat16 template.  A library
-    built before bf16 payloads ignores unknown flags and would read the bf16 template as fp32, so the bit is set only when the
-    library reports TPLATE_BF16=1 in its build configuration."""
+def tplate_flags(bf16, grad_f32=False):
+    """The flag bits that tell the raymarch calls the template's dtype: MVP_FLAG_TPLATE_BF16 for a bfloat16 template, plus
+    MVP_FLAG_GRAD_TPLATE_F32 with grad_f32 (its gradient buffers are fp32 and accumulated in fp32; nothing for an fp32 template,
+    whose gradient is fp32 anyway).  A library built before either feature ignores unknown flags and would read the bf16 template
+    as fp32, or the fp32 gradient buffer as bf16, so each bit is set only when the library reports TPLATE_BF16=1 /
+    GRAD_TPLATE_F32=1 in its build configuration."""
     if not bf16:
         return 0
-    if "TPLATE_BF16=1" not in LIB.mvp_build_config().decode().split():
+    config = LIB.mvp_build_config().decode().split()
+    if "TPLATE_BF16=1" not in config:
         raise RuntimeError("mvpraymarch_b200: this library (%s) does not support bfloat16 templates" % _build.LIB)
-    return FLAG_TPLATE_BF16
+    if not grad_f32:
+        return FLAG_TPLATE_BF16
+    if "GRAD_TPLATE_F32=1" not in config:
+        raise RuntimeError("mvpraymarch_b200: this library (%s) does not accumulate bfloat16 templates' gradients in fp32" % _build.LIB)
+    return FLAG_TPLATE_BF16 | FLAG_GRAD_TPLATE_F32
 
 
 def require_epilogue_bf16():

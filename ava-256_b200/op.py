@@ -10,10 +10,12 @@ everything else (mvpraymarch.py:279-292).  Differences that are deliberate:
     it is kept for backward instead of being rebuilt;
   * 64-bit indexing (the reference overflows int32 at N*K*T^3*4 >= 2^31, primsampler.h:31-36);
   * the template may be bfloat16 (what the decoders produce under torch.autocast): it is rendered exactly as its fp32
-    widening and its gradient is bfloat16, accumulated in bf16 by the backward kernel.  `mvpraymarch` widens bfloat16
-    primpos / primrot / primscale / warp to fp32 before the op (exact; autograd casts their gradients back).  The reference
-    reads a half-precision template as fp32 without checking its dtype (mvpraymarch.cpp:250-272).
+    widening and its gradient is bfloat16, accumulated in bf16 by the backward kernel -- or, on request (`template_grad_dtype`
+    below), accumulated in fp32.  `mvpraymarch` widens bfloat16 primpos / primrot / primscale / warp to fp32 before the op
+    (exact; autograd casts their gradients back).  The reference reads a half-precision template as fp32 without checking its
+    dtype (mvpraymarch.cpp:250-272).
 """
+import contextlib
 import ctypes
 
 import torch
@@ -46,9 +48,52 @@ def _check_f32_cuda(name, t, allow_bf16=False):
         raise RuntimeError("%s must be float32" % name)
 
 
+_TEMPLATE_GRAD = {}   # "dtype": the setting of the innermost active `template_grad_dtype` context
+
+
+def _check_template_grad_dtype(dtype):
+    if dtype is not None and dtype is not torch.float32:
+        raise ValueError("template_grad_dtype must be None (the template's own dtype) or torch.float32, got %r" % (dtype,))
+    return dtype
+
+
+@contextlib.contextmanager
+def template_grad_dtype(dtype):
+    """Within the block, raymarch calls with a bfloat16 template accumulate its gradient in fp32 (dtype=torch.float32) or in the
+    template's own dtype (None, the default).  With fp32 the template is still read as bf16 (same images as without), the backward
+    adds to an fp32 [N,K,TD,TH,TW,4] buffer that the op allocates (twice the bf16 gradient's size, cleared by the forward's render
+    kernel) and every gradient equals that of the fp32 template `template.float()` up to the order of the fp32 atomics.  The op
+    returns that fp32 gradient and autograd casts it to the input's dtype, so `template.grad` stays bfloat16 and holds the fp32
+    sum rounded once; the cast allocates a bf16 temporary of the gradient's size besides the fp32 buffer.  An fp32 template
+    ignores the setting.  The decision is taken by the forward call and kept for its backward, so the backward may run outside the
+    block (autograd runs it on its own thread).  The only way an unmodified caller of `mvpraymarch` opts in:
+
+        with ava256_b200.op.template_grad_dtype(torch.float32):
+            rayrgba = mvpraymarch(raypos, raydir, stepsize, tminmax, primtransf, template_bf16, warp)
+        loss(rayrgba).backward()
+    """
+    _check_template_grad_dtype(dtype)
+    prev = _TEMPLATE_GRAD.get("dtype")
+    _TEMPLATE_GRAD["dtype"] = dtype
+    try:
+        yield
+    finally:
+        _TEMPLATE_GRAD["dtype"] = prev
+
+
+_template_grad_block = template_grad_dtype     # for the functions whose keyword of the same name hides it
+
+
 def _widen_bf16(t):
     """A bfloat16 tensor as fp32 (exact); anything else unchanged, so that other dtypes still meet the op's dtype check."""
     return t.float() if t is not None and t.dtype == torch.bfloat16 else t
+
+
+def _empty_template_grad(template, tflags):
+    """The template's gradient buffer: fp32 with MVP_FLAG_GRAD_TPLATE_F32, else of the template's dtype."""
+    if tflags & _lib.FLAG_GRAD_TPLATE_F32:
+        return torch.empty(template.shape, dtype=torch.float32, device=template.device)
+    return torch.empty_like(template)
 
 
 class MVPRaymarch(Function):
@@ -98,7 +143,8 @@ class MVPRaymarch(Function):
                 _check_f32_cuda(name, t)
         _check_f32_cuda("template", template, allow_bf16=True)
         bf16 = template.dtype == torch.bfloat16                        # MVP_FLAG_TPLATE_BF16: rendered as template.float()
-        tflags = _lib.tplate_flags(bf16)
+        grad_f32 = bf16 and _check_template_grad_dtype(options.get("_template_grad_dtype")) is torch.float32
+        tflags = _lib.tplate_flags(bf16, grad_f32)                     # + MVP_FLAG_GRAD_TPLATE_F32: fp32 template gradient
         if warp is not None:                                           # mvpraymarch.py:124
             assert warp.is_contiguous() and warp.dim() == 6 and warp.size(-1) == 3, \
                 "channels-last warp field [N,K,WD,WH,WW,3] required"
@@ -166,8 +212,8 @@ class MVPRaymarch(Function):
             if gradmode:
                 # The gradient buffers of the backward (mvpraymarch.py:240-246 zeros_like's them there) are made now and zero-filled
                 # by the forward's render kernel on the side (mvp_forward_args::clear_grad_*): no memset pass in the step.
-                grads = [torch.empty_like(primpos), torch.empty_like(primrot), torch.empty_like(primscale), torch.empty_like(template),
-                         torch.empty_like(warp) if usewarp else None]
+                grads = [torch.empty_like(primpos), torch.empty_like(primrot), torch.empty_like(primscale),
+                         _empty_template_grad(template, tflags), torch.empty_like(warp) if usewarp else None]
                 a.clear_grad_primpos, a.clear_grad_primrot, a.clear_grad_primscale = _ptr(grads[0]), _ptr(grads[1]), _ptr(grads[2])
                 a.clear_grad_tplate, a.clear_grad_warp = _ptr(grads[3]), _ptr(grads[4])
             stream = torch.cuda.current_stream(dev).cuda_stream
@@ -219,8 +265,8 @@ def _march_backward(ctx, grad_rayrgba, grad_rayalpha, want_rays):
         grads, ctx.grads = ctx.grads, None
         fresh = grads is not None          # the forward's render kernel zero-filled them; a second backward through the
         if not fresh:                      # same graph (retain_graph) gets new ones, zero-filled by the library
-            grads = [torch.empty_like(primpos), torch.empty_like(primrot), torch.empty_like(primscale), torch.empty_like(template),
-                     torch.empty_like(warp) if usewarp else None]
+            grads = [torch.empty_like(primpos), torch.empty_like(primrot), torch.empty_like(primscale),
+                     _empty_template_grad(template, ctx.tflags), torch.empty_like(warp) if usewarp else None]
         grad_primpos, grad_primrot, grad_primscale, grad_template, grad_warp = grads
         if warp is not None and not usewarp:                       # mvpraymarch.py:246 (zero when algo 0 ignores it)
             grad_warp = torch.zeros_like(warp)
@@ -401,7 +447,7 @@ def mvpraymarch(
         "algo": algo, "usebvh": usebvh, "sortprims": sortprims, "randomorder": randomorder,
         "maxhitboxes": maxhitboxes, "synchitboxes": synchitboxes, "chlast": chlast, "fadescale": fadescale,
         "fadeexp": fadeexp, "accum": accum, "termthresh": termthresh, "griddim": griddim, "blocksize": blocksize,
-        "bwdblocksize": bwdblocksize, "_order": order,
+        "bwdblocksize": bwdblocksize, "_order": order, "_template_grad_dtype": _TEMPLATE_GRAD.get("dtype"),
     }
     if _CAMERA.get("cam") is not None:
         options["_camera"] = _CAMERA["cam"]
@@ -433,7 +479,7 @@ def mvpraymarch_planes(*args, **kwargs):
 
 
 def mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, volradius, stepsize, primtransf, template, warp, planes=False,
-                       camera_grad=False, **kwargs):
+                       camera_grad=False, template_grad_dtype=None, **kwargs):
     """`compute_raydirs` + `mvpraymarch` of models/autoencoder.py:240-252 as ONE call: the first six parameters are those of the
     reference's compute_raydirs (extensions/utils/utils.py:48-51), the rest those of `mvpraymarch` after its ray arguments.
 
@@ -447,7 +493,13 @@ def mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, volradius,
     the gradient of the image with every discrete decision of the march held fixed (C-ABI mvp_raymarch_backward_rays, then the ray
     generator's adjoint mvp_compute_raydirs_backward); pixelcoords and volradius get none.  When no camera tensor requires grad,
     the plain backward runs.
+    template_grad_dtype=torch.float32 accumulates a bfloat16 template's gradient in fp32 (see the `template_grad_dtype` context
+    manager); None leaves the setting of an enclosing `template_grad_dtype` block, by default the template's own dtype.
     Returns rayrgba [N,H,W,4], or (rayrgb [N,3,H,W], rayalpha [N,1,H,W]) with planes=True."""
+    if _check_template_grad_dtype(template_grad_dtype) is not None:
+        with _template_grad_block(template_grad_dtype):
+            return mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, volradius, stepsize, primtransf, template, warp,
+                                      planes=planes, camera_grad=camera_grad, **kwargs)
     march = mvpraymarch_planes if planes else mvpraymarch
     grad = bool(camera_grad) and torch.is_grad_enabled() and any(t.requires_grad for t in (viewpos, viewrot, focal, princpt))
     if grad:

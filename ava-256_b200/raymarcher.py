@@ -2,23 +2,35 @@
 same forward signature and return tuple).  The image planes `rayrgb` / `rayalpha` come straight out of the render kernel's
 epilogue and their gradients go straight into the backward's prologue (`op.mvpraymarch_planes`); the reference makes them
 with a permute + two `.contiguous()` copies (:50-51)."""
+import contextlib
+
 import torch.nn as nn
 
 from .composite import split_rgba
-from .op import mvpraymarch, mvpraymarch_camera, mvpraymarch_planes
+from .op import _check_template_grad_dtype, mvpraymarch, mvpraymarch_camera, mvpraymarch_planes, template_grad_dtype
 
 
 class Raymarcher(nn.Module):
-    def __init__(self, volradius, dt: float = 1.0, with_rgba: bool = False):
+    def __init__(self, volradius, dt: float = 1.0, with_rgba: bool = False, template_grad_dtype=None):
         """with_rgba: also return the [N,4,H,W] view of the channels-last `rayrgba` as the third item, like the reference
         (:50).  No caller in ava-256 reads it (models/autoencoder.py:246 drops it), so by default the channels-last image
-        is never written and the third item is None."""
+        is never written and the third item is None.
+        template_grad_dtype: torch.float32 accumulates a bfloat16 template's gradient in fp32 in `forward` and `forward_camera`
+        (see `op.template_grad_dtype`); None (default) leaves it to the template's dtype or an enclosing `op.template_grad_dtype`."""
         super().__init__()
         self.volume_radius = volradius
         self.dt = dt / self.volume_radius                       # mvpraymarcher.py:24
         self.with_rgba = with_rgba
+        self.template_grad_dtype = _check_template_grad_dtype(template_grad_dtype)
+
+    def _grad_dtype(self):
+        return contextlib.nullcontext() if self.template_grad_dtype is None else template_grad_dtype(self.template_grad_dtype)
 
     def forward(self, raypos, raydir, tminmax, decout, renderoptions={}, rayterm=None, with_pos_img=None):
+        with self._grad_dtype():
+            return self._forward(raypos, raydir, tminmax, decout, renderoptions, rayterm)
+
+    def _forward(self, raypos, raydir, tminmax, decout, renderoptions, rayterm):
         args = (raypos, raydir, self.dt, tminmax, (decout["primpos"], decout["primrot"], decout["primscale"]))
         kwargs = dict(template=decout["template"], warp=decout["warp"] if "warp" in decout else None, rayterm=rayterm,
                       **{k: v for k, v in renderoptions.items() if k in mvpraymarch.__code__.co_varnames})   # :45
@@ -38,7 +50,7 @@ class Raymarcher(nn.Module):
         out = mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, self.volume_radius, self.dt,
                                  (decout["primpos"], decout["primrot"], decout["primscale"]), decout["template"],
                                  decout["warp"] if "warp" in decout else None, planes=not self.with_rgba, camera_grad=camera_grad,
-                                 **kwargs)
+                                 template_grad_dtype=self.template_grad_dtype, **kwargs)
         if self.with_rgba:
             rayrgb, rayalpha = split_rgba(out)
             return rayrgb, rayalpha, out.permute(0, 3, 1, 2), None

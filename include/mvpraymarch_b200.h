@@ -59,7 +59,8 @@ extern "C" {
 #define MVP_ERR_WORKSPACE (-4) /* workspace too small or misaligned (256 B) */
 #define MVP_ERR_ALGO (-5)      /* algo must be 0 (no warp field) or 1 (warp field, primsampler.h:53-58) */
 #define MVP_ERR_ALIGN (-6)     /* a vector-accessed buffer is misaligned: tplate, rayrgba, grad_rayrgba, grad_tplate, rayaux,
-                                * clear_grad_* need 16 bytes (tplate, grad_tplate 8 with MVP_FLAG_TPLATE_BF16), tminmax 8,
+                                * clear_grad_* need 16 bytes (tplate, grad_tplate 8 with MVP_FLAG_TPLATE_BF16; grad_tplate 16
+                                * again with MVP_FLAG_GRAD_TPLATE_F32), tminmax 8,
                                 * everything else 4 */
 #define MVP_ERR_STRUCT (-7)    /* args->struct_size != sizeof(the struct this library was built with) */
 #define MVP_ERR_CAMERA (-8)    /* camera.volradius must be finite and > 0 */
@@ -82,6 +83,15 @@ typedef struct mvp_shape {
                                  * template; grad_tplate is accumulated in bf16 (round to nearest even per reduction).  Everything
                                  * else stays fp32.  Must be the same in a forward and the backward that follows it.  The library
                                  * supports it iff mvp_build_config() lists TPLATE_BF16=1 (an older one ignores the bit). */
+#define MVP_FLAG_GRAD_TPLATE_F32 16u /* forward and backward, with MVP_FLAG_TPLATE_BF16: the template is still read as bfloat16, but
+                                 * grad_tplate and clear_grad_tplate point to FP32 buffers [N,K,TD,TH,TW,4] (16 bytes per voxel,
+                                 * 16-byte aligned) and the backward accumulates into them with fp32 reductions, like the fp32
+                                 * kernels: every gradient, the template's included, is that of the fp32 kernels on the widened
+                                 * template up to the order of the fp32 atomics, and images, raysat and rayaux are those of the bf16
+                                 * path.  Without MVP_FLAG_TPLATE_BF16 it changes nothing (an fp32 template's gradient is fp32).
+                                 * Like MVP_FLAG_TPLATE_BF16 it must be the same in a forward and the backward that follows it: the
+                                 * forward sizes its clear of clear_grad_tplate by it.  The library supports it iff
+                                 * mvp_build_config() lists GRAD_TPLATE_F32=1 (an older one ignores the bit). */
 #define MVP_FLAG_TEST_TINY_LISTS 0x100u /* test hook: forward keeps at most 16 saved tile-list entries per view, so almost
                                  * every tile takes the backward's rebuild path */
 
