@@ -2372,19 +2372,28 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         const int nxt = __ffs(grp & ~((2u << lane) - 1u)) - 1;          // next lane of the group, -1: none
                         const int nst = 32 - __clz(__reduce_max_sync(0xffffffffu, act ? __popc(grp) : 1) - 1);   // ceil(log2(largest group))
                         float *gc = gslab + (size_t)base * Payload<V>::kWords;
+                        // Two corners (the lower and upper x voxel of one y/z edge) share each jumping loop: half the loops and
+                        // the pointer shuffles, and two independent shuffle chains in flight per stage.
 #pragma unroll
-                        for (int cn = 0; cn < 8; ++cn) {
-                            const int o = ((cn & 1) ? sx : 0) + ((cn & 2) ? sy : 0) + ((cn & 4) ? sz : 0);
-                            const float w_ = (wx_[cn & 1] * wy_[(cn >> 1) & 1]) * wz_[(cn >> 2) & 1];   // same product as above
-                            float ua = w_ * d0, ub = w_ * d1, uc = w_ * d2, ud = w_ * B;
+                        for (int cn = 0; cn < 8; cn += 2) {
+                            const int o = ((cn & 2) ? sy : 0) + ((cn & 4) ? sz : 0);
+                            const float wyz = wy_[(cn >> 1) & 1], wzz = wz_[(cn >> 2) & 1];
+                            const float w0 = (wx_[0] * wyz) * wzz, w1 = (wx_[1] * wyz) * wzz;    // same products as above
+                            float ua = w0 * d0, ub = w0 * d1, uc = w0 * d2, ud = w0 * B;
+                            float ea = w1 * d0, eb = w1 * d1, ec = w1 * d2, ed = w1 * B;
                             for (int s = 0, nx = nxt; s < nst; ++s) {
                                 const int src = nx >= 0 ? nx : lane;
                                 const float va = __shfl_sync(0xffffffffu, ua, src), vb = __shfl_sync(0xffffffffu, ub, src);
                                 const float vc = __shfl_sync(0xffffffffu, uc, src), vd = __shfl_sync(0xffffffffu, ud, src);
-                                if (nx >= 0) { ua += va; ub += vb; uc += vc; ud += vd; }
+                                const float fa = __shfl_sync(0xffffffffu, ea, src), fb = __shfl_sync(0xffffffffu, eb, src);
+                                const float fc = __shfl_sync(0xffffffffu, ec, src), fd = __shfl_sync(0xffffffffu, ed, src);
+                                if (nx >= 0) { ua += va; ub += vb; uc += vc; ud += vd; ea += fa; eb += fb; ec += fc; ed += fd; }
                                 nx = __shfl_sync(0xffffffffu, nx, src);
                             }
-                            if (lead) Payload<V>::red(gc, (size_t)o, ua, ub, uc, ud);
+                            if (lead) {
+                                Payload<V>::red(gc, (size_t)o, ua, ub, uc, ud);
+                                Payload<V>::red(gc, (size_t)(o + sx), ea, eb, ec, ed);
+                            }
                         }
 #if defined(MVP_CPU_EMUL) && defined(MVP_EMUL_STATS)
                         // [7] payload-gradient reductions issued; g_emul_bwd_groups[g - 1]: cell groups of g samples;
