@@ -2006,8 +2006,14 @@ __device__ __forceinline__ int *ray_steps(BwdWarpSmem<CAP> *S) {
     else return nullptr;
 }
 
-template <int T, int CAP, bool kWarp, typename V, bool kRayGrad>
+// Gradient set of a backward kernel: what it computes besides the (optional, kRayGrad) ray gradients.
+constexpr int kGradAll = 0;         // transforms, template (+ warp field)
+constexpr int kGradNoPayload = 1;   // transforms only (MVP_FLAG_NO_TPLATE_GRAD): no payload-gradient scatter
+constexpr int kGradRaysOnly = 2;    // ray gradients only (MVP_FLAG_RAY_GRADS_ONLY; kRayGrad kernels): no transform sums either
+
+template <int T, int CAP, bool kWarp, typename V, bool kRayGrad, int kSet>
 __device__ __forceinline__ bool backward_tile(const Params &p, const int n, const int tx, const int ty, const int lane, BwdWarpSmem<CAP> *const S) {
+    static_assert(kSet != kGradRaysOnly || kRayGrad, "a rays-only backward computes the ray gradients");
     int *const sk = S->k, *const siv = S->iv;
     RowEntry *const sstage = S->stage;
     unsigned long long *const sbar = S->bar;
@@ -2207,12 +2213,15 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
 #endif
                 if (maxlen <= 0) continue;
                 const V *slab = reinterpret_cast<const V *>(p.tplate) + (pvK + k) * slabsz;
-                float *gslab = p.g_tplate + (pvK + k) * slabsz * Payload<V>::kWords;   // as 4-byte words, see Payload
+                // as 4-byte words, see Payload (kGradAll only: the other sets do not touch p.g_tplate)
+                float *gslab = kSet == kGradAll ? p.g_tplate + (pvK + k) * slabsz * Payload<V>::kWords : nullptr;
                 // transform-gradient accumulators of THIS lane for this slab: Gx[i][j] = sum xm_i * dL/dy_j and
                 // Gy[j] = sum dL/dy_j; grad_rot/scale/pos are linear in them (derived once per slab, before the reduction)
 #if MVP_BWD_LANESMEM
+                if (kSet != kGradRaysOnly) {
 #pragma unroll
-                for (int i = 0; i < 12; ++i) L_GX(i) = 0.f;
+                    for (int i = 0; i < 12; ++i) L_GX(i) = 0.f;
+                }
 #else
                 float gx[9], gsum[3];
 #pragma unroll
@@ -2300,8 +2309,9 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         const bool issat = (meta & 256) != 0;
                         // Without a warp field, lanes past the end of a short batch stay until the payload-gradient merge below
                         // (warp-wide collectives).  They carry lane 0's sample, so every address they form is valid; they
-                        // scatter nothing and leave before the transform-gradient sums.
-                        if (kWarp && !act) continue;
+                        // scatter nothing and leave before the transform-gradient sums.  The reduced gradient sets have no
+                        // merge, so there they leave here.
+                        if ((kWarp || kSet != kGradAll) && !act) continue;
                         // per-ray data of the owner lane
                         const float *pr_ = sray + owner;
                         const float oLx = pr_[0 * 32], oLy = pr_[1 * 32], oLz = pr_[2 * 32], oLw = pr_[3 * 32];
@@ -2367,6 +2377,8 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         // reductions.  So the lanes of one cell are summed first, by pointer jumping within the group (at stage
                         // s every lane adds the partial sum of the member 2^s places after it, then takes over that member's
                         // successor), and only the group's lowest lane, which then holds the total, issues the 8 reductions.
+                        // The reduced gradient sets compile all of it out.
+                        if constexpr (kSet == kGradAll) {
                         const unsigned grp = match_any_warp(act ? base : -1);
                         const bool lead = act && (grp & ((1u << lane) - 1u)) == 0u;
                         const int nxt = __ffs(grp & ~((2u << lane) - 1u)) - 1;          // next lane of the group, -1: none
@@ -2417,6 +2429,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                             __syncwarp();
                         }
 #endif
+                        }
                         if (!act) continue;
                         // dL/d(index): d(weight)/d(index) is +1 on the upper corner, -1 on the lower one; on a clamped axis
                         // the reference sees the upper voxel as ITS lower corner (sign -1) and no other corner.
@@ -2431,7 +2444,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         // ---- algo 1 (PrimSamplerTW<true>): payload sampled at the warp-field-displaced position ----
                         const size_t wsl = (size_t)p.WD * p.WH * p.WW * 3;
                         const float *wk = p.warp + ((size_t)(n * p.pview) * p.K + k) * wsl;
-                        float *gwk = p.g_warp + ((size_t)(n * p.pview) * p.K + k) * wsl;
+                        float *gwk = kSet == kGradAll ? p.g_warp + ((size_t)(n * p.pview) * p.K + k) * wsl : nullptr;
                         const float e1 = p.fadeexp - 1.f;
                         const float pw0 = __powf(fabsf(y0), e1), pw1 = __powf(fabsf(y1), e1), pw2 = __powf(fabsf(y2), e1);
                         const float fade = __expf(-p.fadescale * (pw0 * fabsf(y0) + pw1 * fabsf(y1) + pw2 * fabsf(y2)));
@@ -2470,9 +2483,11 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         gy0 = cf * pw0 * (y0 > 0.f ? 1.f : -1.f);
                         gy1 = cf * pw1 * (y1 > 0.f ? 1.f : -1.f);
                         gy2 = cf * pw2 * (y2 > 0.f ? 1.f : -1.f);
+                        if constexpr (kSet == kGradAll) {
 #pragma unroll
                         for (int cn = 0; cn < 8; ++cn)
                             if (ct.idx[cn] >= 0) Payload<V>::red(gslab, (size_t)ct.idx[cn], ct.w[cn] * d0, ct.w[cn] * d1, ct.w[cn] * d2, ct.w[cn] * B);
+                        }
                         // dL/d(warped position)  (utils.h:591-642), then through the warp field (primsampler.h:82-88)
                         const float e0 = gmx * (A * gp0 + B * ga0), e1_ = gmy * (A * gp1 + B * ga1), e2 = gmz * (A * gp2 + B * ga2);
                         float h0 = 0.f, h1 = 0.f, h2 = 0.f;
@@ -2480,8 +2495,10 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         for (int cn = 0; cn < 8; ++cn) {
                             if (cw.idx[cn] >= 0) {
                                 const float *v = wk + (size_t)cw.idx[cn] * 3;
-                                float *gv = gwk + (size_t)cw.idx[cn] * 3;
-                                atomicAdd(gv, cw.w[cn] * e0); atomicAdd(gv + 1, cw.w[cn] * e1_); atomicAdd(gv + 2, cw.w[cn] * e2);
+                                if constexpr (kSet == kGradAll) {
+                                    float *gv = gwk + (size_t)cw.idx[cn] * 3;
+                                    atomicAdd(gv, cw.w[cn] * e0); atomicAdd(gv + 1, cw.w[cn] * e1_); atomicAdd(gv + 2, cw.w[cn] * e2);
+                                }
                                 const float dpw = __ldg(v) * e0 + __ldg(v + 1) * e1_ + __ldg(v + 2) * e2;
                                 const float wx = (cn & 1) ? cw.x0 : cw.x1, wy = (cn & 2) ? cw.y0 : cw.y1, wz = (cn & 4) ? cw.z0 : cw.z1;
                                 h0 += ((cn & 1) ? dpw : -dpw) * (wy * wz);
@@ -2499,6 +2516,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                             atomicAdd(o + 3 * 32, jf * gy0); atomicAdd(o + 4 * 32, jf * gy1); atomicAdd(o + 5 * 32, jf * gy2);
                         }
                         // ---- primtransf.h:155-179, accumulated in factored form ----
+                        if (kSet != kGradRaysOnly) {
 #if MVP_BWD_LANESMEM
                         L_GX(0) = L_GX(0) + xm * gy0; L_GX(1) = L_GX(1) + xm * gy1; L_GX(2) = L_GX(2) + xm * gy2;
                         L_GX(3) = L_GX(3) + ym * gy0; L_GX(4) = L_GX(4) + ym * gy1; L_GX(5) = L_GX(5) + ym * gy2;
@@ -2510,6 +2528,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         gx[6] += zm * gy0; gx[7] += zm * gy1; gx[8] += zm * gy2;
                         gsum[0] += gy0; gsum[1] += gy1; gsum[2] += gy2;
 #endif
+                        }
                     }
                 }
                 if (!__any_sync(0xffffffffu, touched)) continue;
@@ -2519,9 +2538,11 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
 #endif
 #if MVP_BWD_LANESMEM
                 float gx[9], gsum[3];
+                if (kSet != kGradRaysOnly) {
 #pragma unroll
-                for (int i = 0; i < 9; ++i) gx[i] = L_GX(i);
-                gsum[0] = L_GX(9); gsum[1] = L_GX(10); gsum[2] = L_GX(11);
+                    for (int i = 0; i < 9; ++i) gx[i] = L_GX(i);
+                    gsum[0] = L_GX(9); gsum[1] = L_GX(10); gsum[2] = L_GX(11);
+                }
 #endif
                 if (kRayGrad) {
                     // the owner's slab sums to world coordinates, dL/dx = R (s * dL/dy), into the ray's totals; cleared for the next slab
@@ -2539,6 +2560,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                     ra[5 * 32] += q.r20 * b0 + q.r21 * b1 + q.r22 * b2;
                     __syncwarp();
                 }
+                if (kSet == kGradRaysOnly) continue;      // no transform gradients: no butterfly, no atomics
                 float g[16];
                 g[0] = q.r00 * gx[0] + q.r10 * gx[3] + q.r20 * gx[6];
                 g[1] = q.r01 * gx[1] + q.r11 * gx[4] + q.r21 * gx[7];
@@ -2600,8 +2622,8 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
 }
 
 // kRayGrad: also write the per-ray gradients p.g_raypos / g_raydir / g_tminmax (mvp_raymarch_backward_rays); false compiles to
-// the plain backward
-template <int T, int CAP, bool kWarp, typename V, bool kRayGrad = false>
+// the plain backward.  kSet: the gradient set (kGradAll, kGradNoPayload, kGradRaysOnly); the default is the full backward.
+template <int T, int CAP, bool kWarp, typename V, bool kRayGrad = false, int kSet = kGradAll>
 __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_BWD_MINB * 4) / kWarps : 12 / kWarps) render_backward_kernel(const Params p) {
     __shared__ typename BwdSmemOf<CAP, kRayGrad>::type s_w[kWarps];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -2611,7 +2633,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         for (int i = blockIdx.x * kWarps + warp; i < cnt; i += gridDim.x * kWarps) {
             const int id = p.heavylist[i];
             const int tx = id % p.TXn, ty = (id / p.TXn) % p.TYn, n = id / (p.TXn * p.TYn);
-            backward_tile<T, CAP, kWarp, V, kRayGrad>(p, n, tx, ty, lane, S);
+            backward_tile<T, CAP, kWarp, V, kRayGrad, kSet>(p, n, tx, ty, lane, S);
             __syncwarp();
         }
     } else {
@@ -2624,7 +2646,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         const int tx = blockIdx.x * kBlkTX + (warp % kBlkTX), ty = blockIdx.y * kBlkTY + (warp / kBlkTX), n = blockIdx.z;
 #endif
         if (tx >= p.TXn || ty >= p.TYn) return;
-        if (!backward_tile<T, CAP, kWarp, V, kRayGrad>(p, n, tx, ty, lane, S) && lane == 0)
+        if (!backward_tile<T, CAP, kWarp, V, kRayGrad, kSet>(p, n, tx, ty, lane, S) && lane == 0)
             p.heavylist[atomicAdd(p.heavycnt, 1)] = (n * p.TYn + ty) * p.TXn + tx;
     }
 }
@@ -2846,7 +2868,7 @@ const char *mvp_build_config(void) {
     return "LIST_REUSE=" MVP_STR(MVP_LIST_REUSE)
            " LIST_MARGIN=" MVP_STR(MVP_LIST_MARGIN) " XBUCKETS=" MVP_STR(MVP_XBUCKETS) " FASTCAP=" MVP_STR(MVP_FWD_FASTCAP) "/" MVP_STR(MVP_BWD_FASTCAP) " SMEM_UNION=" MVP_STR(MVP_SMEM_UNION) " CARVEOUT=" MVP_STR(MVP_FWD_CARVEOUT) "/" MVP_STR(MVP_BWD_CARVEOUT) " FWD_RING=" MVP_STR(MVP_FWD_RING) " BWD_SMEMREC=" MVP_STR(MVP_BWD_SMEMREC) " BWD_LANESMEM=" MVP_STR(MVP_BWD_LANESMEM) " CTA_ORDER=" MVP_STR(MVP_CTA_ORDER) " CTA_ORDER_MIN=" MVP_STR(MVP_CTA_ORDER_MIN)
            " CHUNK=" MVP_STR(MVP_CHUNK) " FWD_MINB=" MVP_STR(MVP_FWD_MINB) " BWD_MINB=" MVP_STR(MVP_BWD_MINB)
-           " WARPS=" MVP_STR(MVP_WARPS) " BLK_TX=" MVP_STR(MVP_BLK_TX) " TPLATE_BF16=1 EPILOGUE_BF16=1 RAY_GRADS=1 GRAD_TPLATE_F32=1"
+           " WARPS=" MVP_STR(MVP_WARPS) " BLK_TX=" MVP_STR(MVP_BLK_TX) " TPLATE_BF16=1 EPILOGUE_BF16=1 RAY_GRADS=1 GRAD_TPLATE_F32=1 GRAD_SELECT=1"
 #ifdef MVP_CPU_EMUL
            " CPU_EMUL"
 #endif
@@ -2938,6 +2960,11 @@ int mvp_backward_launch_count(uint32_t flags) { return (flags & MVP_FLAG_ACCEL_V
 
 static inline bool misaligned(const void *p, uintptr_t a) { return p && ((uintptr_t)p & (a - 1)); }
 
+// The gradient buffers a call's flags request: MVP_FLAG_NO_TPLATE_GRAD drops the template's and the warp field's,
+// MVP_FLAG_RAY_GRADS_ONLY every primitive gradient.  A buffer that is not requested is neither read nor written.
+static inline bool wants_tplate_grad(uint32_t flags) { return !(flags & (MVP_FLAG_NO_TPLATE_GRAD | MVP_FLAG_RAY_GRADS_ONLY)); }
+static inline bool wants_transform_grad(uint32_t flags) { return !(flags & MVP_FLAG_RAY_GRADS_ONLY); }
+
 // 4-byte words per voxel of the template gradient: bf16 (2) only for a bf16 template without MVP_FLAG_GRAD_TPLATE_F32
 static inline unsigned grad_tplate_words(uint32_t flags) {
     return ((flags & MVP_FLAG_TPLATE_BF16) && !(flags & MVP_FLAG_GRAD_TPLATE_F32)) ? Payload<Bf16x4>::kWords : Payload<float4>::kWords;
@@ -2961,15 +2988,20 @@ int mvp_raymarch_forward(const mvp_forward_args *a, void *stream) {
     if (!(a->stepsize > 0.f) || !(a->stepsize < 3.0e38f)) return MVP_ERR_STEPSIZE;
     const Layout L = make_layout(a->shape);
     if (a->workspace_bytes < L.total || ((uintptr_t)a->workspace & 255)) return MVP_ERR_WORKSPACE;
+    // the clear_grad_* buffers the flags request (the others are ignored, whatever they point to)
+    const bool gt = wants_tplate_grad(a->flags), gp = wants_transform_grad(a->flags);
+    float *const clr_primpos = gp ? a->clear_grad_primpos : nullptr, *const clr_primrot = gp ? a->clear_grad_primrot : nullptr;
+    float *const clr_primscale = gp ? a->clear_grad_primscale : nullptr;
+    float *const clr_tplate = gt ? a->clear_grad_tplate : nullptr, *const clr_warp = gt ? a->clear_grad_warp : nullptr;
     // vector accesses: float4 (tplate, rayrgba; a bf16 tplate 8 bytes per voxel), int4 (rayaux), float2 (tminmax); everything else
     // is read as scalars.  The clear_grad_* buffers are zero-filled with 16-byte stores whatever the payload type.
     const bool bf16 = (a->flags & MVP_FLAG_TPLATE_BF16) != 0;
     if (misaligned(a->tplate, bf16 ? 8 : 16) || misaligned(a->rayrgba, 16) || misaligned(a->rayaux, 16) || misaligned(a->tminmax, 8) ||
         misaligned(a->raypos, 4) || misaligned(a->raydir, 4) || misaligned(a->primpos, 4) || misaligned(a->primrot, 4) ||
         misaligned(a->primscale, 4) || misaligned(a->raysat, 4) || misaligned(a->warp, 4) || misaligned(a->rayrgb_nchw, 4) ||
-        misaligned(a->rayalpha_nchw, 4) || misaligned(a->order, 4) || misaligned(a->clear_grad_primpos, 16) ||
-        misaligned(a->clear_grad_primrot, 16) || misaligned(a->clear_grad_primscale, 16) || misaligned(a->clear_grad_tplate, 16) ||
-        misaligned(a->clear_grad_warp, 16))
+        misaligned(a->rayalpha_nchw, 4) || misaligned(a->order, 4) || misaligned(clr_primpos, 16) ||
+        misaligned(clr_primrot, 16) || misaligned(clr_primscale, 16) || misaligned(clr_tplate, 16) ||
+        misaligned(clr_warp, 16))
         return MVP_ERR_ALIGN;
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)a->workspace;
@@ -3004,8 +3036,7 @@ int mvp_raymarch_forward(const mvp_forward_args *a, void *stream) {
     if (a->raysat) {
         // gradient buffers to clear for the coming backward: in the fast render kernel (one slice per warp), see clear_grad_slices
         const size_t nk = (size_t)(pview ? a->shape.N : 1) * a->shape.K;
-        float *const bufs[kClearBufs] = {a->clear_grad_primpos, a->clear_grad_primrot, a->clear_grad_primscale, a->clear_grad_tplate,
-                                         a->algo == 1 ? a->clear_grad_warp : nullptr};
+        float *const bufs[kClearBufs] = {clr_primpos, clr_primrot, clr_primscale, clr_tplate, a->algo == 1 ? clr_warp : nullptr};
         // sizes in 4-byte words: a bf16 template gradient holds two channels per word
         const size_t floats[kClearBufs] = {nk * 3, nk * 9, nk * 3, nk * a->shape.TD * a->shape.TH * a->shape.TW * grad_tplate_words(a->flags),
                                            a->algo == 1 ? nk * a->WD * a->WH * a->WW * 3 : 0};
@@ -3062,9 +3093,16 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
     const int camrc = check_camera(a->camera);
     if (camrc < 0) return camrc;
     const mvp_camera *const camera = camrc ? &a->camera : nullptr;
+    // the gradient set: MVP_FLAG_RAY_GRADS_ONLY needs the ray outputs (without them nothing would be computed)
+    const bool gt = wants_tplate_grad(a->flags), gp = wants_transform_grad(a->flags);
+    if (!gp && !rays) return MVP_ERR_NULL;
+    const int set = !gp ? kGradRaysOnly : (!gt ? kGradNoPayload : kGradAll);
+    float *const grad_primpos = gp ? a->grad_primpos : nullptr, *const grad_primrot = gp ? a->grad_primrot : nullptr;
+    float *const grad_primscale = gp ? a->grad_primscale : nullptr;
+    float *const grad_tplate = gt ? a->grad_tplate : nullptr, *const grad_warp = gt ? a->grad_warp : nullptr;
     if ((!camera && (!a->raypos || !a->raydir || !a->tminmax)) || !a->primpos || !a->primrot || !a->primscale || !a->tplate ||
-        !a->raysat || !a->rayaux || !a->grad_primpos || !a->grad_primrot || !a->grad_primscale ||
-        !a->grad_tplate || !a->workspace)
+        !a->raysat || !a->rayaux || (gp && (!grad_primpos || !grad_primrot || !grad_primscale)) || (gt && !grad_tplate) ||
+        !a->workspace)
         return MVP_ERR_NULL;
     // the image gradient: channels-last [N,H,W,4], or as image planes (both of them, and then not the other form)
     if ((a->grad_rayrgb_nchw == nullptr) != (a->grad_rayalpha_nchw == nullptr)) return MVP_ERR_NULL;
@@ -3072,16 +3110,17 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
     int rc = check_shape(a->shape);
     if (rc != MVP_OK) return rc;
     if (a->algo != 0 && a->algo != 1) return MVP_ERR_ALGO;
-    if (a->algo == 1 && (!a->warp || !a->grad_warp || a->WD < 1 || a->WH < 1 || a->WW < 1)) return (a->warp && a->grad_warp) ? MVP_ERR_SHAPE : MVP_ERR_NULL;
+    if (a->algo == 1 && (!a->warp || (gt && !grad_warp) || a->WD < 1 || a->WH < 1 || a->WW < 1))
+        return (a->warp && (grad_warp || !gt)) ? MVP_ERR_SHAPE : MVP_ERR_NULL;
     if (!(a->stepsize > 0.f) || !(a->stepsize < 3.0e38f)) return MVP_ERR_STEPSIZE;
     const Layout L = make_layout(a->shape);
     if (a->workspace_bytes < L.total || ((uintptr_t)a->workspace & 255)) return MVP_ERR_WORKSPACE;
     const bool bf16 = (a->flags & MVP_FLAG_TPLATE_BF16) != 0;
     const unsigned gwords = grad_tplate_words(a->flags);
-    if (misaligned(a->tplate, bf16 ? 8 : 16) || misaligned(a->grad_tplate, gwords * 4) || misaligned(a->grad_rayrgba, 16) || misaligned(a->rayaux, 16) ||
+    if (misaligned(a->tplate, bf16 ? 8 : 16) || misaligned(grad_tplate, gwords * 4) || misaligned(a->grad_rayrgba, 16) || misaligned(a->rayaux, 16) ||
         misaligned(a->tminmax, 8) || misaligned(a->raypos, 4) || misaligned(a->raydir, 4) || misaligned(a->primpos, 4) ||
-        misaligned(a->primrot, 4) || misaligned(a->primscale, 4) || misaligned(a->raysat, 4) || misaligned(a->grad_primpos, 4) ||
-        misaligned(a->grad_primrot, 4) || misaligned(a->grad_primscale, 4) || misaligned(a->warp, 4) || misaligned(a->grad_warp, 4) ||
+        misaligned(a->primrot, 4) || misaligned(a->primscale, 4) || misaligned(a->raysat, 4) || misaligned(grad_primpos, 4) ||
+        misaligned(grad_primrot, 4) || misaligned(grad_primscale, 4) || misaligned(a->warp, 4) || misaligned(grad_warp, 4) ||
         misaligned(a->grad_rayrgb_nchw, 4) || misaligned(a->grad_rayalpha_nchw, 4) || misaligned(a->order, 4) ||
         misaligned(grad_raypos, 4) || misaligned(grad_raydir, 4) || misaligned(grad_tminmax, 8))
         return MVP_ERR_ALIGN;
@@ -3092,14 +3131,15 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
         rc = launch_accel(a->shape, pview, a->order, a->raypos, a->raydir, camera, a->primpos, a->primrot, a->primscale, ws, L, st);
         if (rc != MVP_OK) return rc;
     }
-    if (a->flags & MVP_FLAG_ZERO_GRADS) {
+    if (a->flags & MVP_FLAG_ZERO_GRADS) {     // the requested buffers only
         const size_t nk = (size_t)(pview ? a->shape.N : 1) * a->shape.K;
-        cudaError_t z = cudaMemsetAsync(a->grad_primpos, 0, nk * 3 * sizeof(float), st);
-        if (z == cudaSuccess) z = cudaMemsetAsync(a->grad_primrot, 0, nk * 9 * sizeof(float), st);
-        if (z == cudaSuccess) z = cudaMemsetAsync(a->grad_primscale, 0, nk * 3 * sizeof(float), st);
-        if (z == cudaSuccess)
-            z = cudaMemsetAsync(a->grad_tplate, 0, nk * a->shape.TD * a->shape.TH * a->shape.TW * gwords * sizeof(float), st);
-        if (z == cudaSuccess && a->algo == 1) z = cudaMemsetAsync(a->grad_warp, 0, nk * a->WD * a->WH * a->WW * 3 * sizeof(float), st);
+        cudaError_t z = cudaSuccess;
+        if (gp) z = cudaMemsetAsync(grad_primpos, 0, nk * 3 * sizeof(float), st);
+        if (gp && z == cudaSuccess) z = cudaMemsetAsync(grad_primrot, 0, nk * 9 * sizeof(float), st);
+        if (gp && z == cudaSuccess) z = cudaMemsetAsync(grad_primscale, 0, nk * 3 * sizeof(float), st);
+        if (gt && z == cudaSuccess)
+            z = cudaMemsetAsync(grad_tplate, 0, nk * a->shape.TD * a->shape.TH * a->shape.TW * gwords * sizeof(float), st);
+        if (gt && z == cudaSuccess && a->algo == 1) z = cudaMemsetAsync(grad_warp, 0, nk * a->WD * a->WH * a->WW * 3 * sizeof(float), st);
         if (z != cudaSuccess) return (int)z;
     }
     Params p{};
@@ -3111,8 +3151,8 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
     p.order = a->order; p.rankof = a->order ? reinterpret_cast<const int *>(ws + L.rankof) : nullptr;
     p.g_rgb_nchw = a->grad_rayrgb_nchw; p.g_alpha_nchw = a->grad_rayalpha_nchw;
     p.grad_rayrgba = a->grad_rayrgba; p.raysat_in = a->raysat; p.rayaux_in = reinterpret_cast<const int4 *>(a->rayaux);
-    p.g_primpos = a->grad_primpos; p.g_primrot = a->grad_primrot; p.g_primscale = a->grad_primscale; p.g_tplate = a->grad_tplate;
-    p.warp = a->warp; p.g_warp = a->grad_warp; p.WD = a->WD; p.WH = a->WH; p.WW = a->WW;
+    p.g_primpos = grad_primpos; p.g_primrot = grad_primrot; p.g_primscale = grad_primscale; p.g_tplate = grad_tplate;
+    p.warp = a->warp; p.g_warp = grad_warp; p.WD = a->WD; p.WH = a->WH; p.WW = a->WW;
     p.g_raypos = grad_raypos; p.g_raydir = grad_raydir; p.g_tminmax = reinterpret_cast<float2 *>(grad_tminmax);
 #if MVP_CTA_ORDER
     dim3 grid((unsigned)((size_t)p.CXn * p.CYn * a->shape.N));
@@ -3139,17 +3179,33 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
             MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV>);                                  \
         }                                                                                                    \
     } while (0)
-#define MVP_LAUNCH_BWD_T(VV)                                                                     \
-    do {                                                                                         \
-        if (a->algo == 1) MVP_LAUNCH_BWD(0, true, VV);                                           \
-        else if (cubic == 8) MVP_LAUNCH_BWD(8, false, VV);                                       \
-        else if (cubic == 16) MVP_LAUNCH_BWD(16, false, VV);                                     \
-        else MVP_LAUNCH_BWD(0, false, VV);                                                       \
+    // the reduced gradient sets (float4 and Bf16x4 only: without a template gradient Bf16x4G32 is Bf16x4)
+#define MVP_LAUNCH_BWD_SET(TT, WW_, VV, RG, SET)                                                             \
+    do {                                                                                                     \
+        MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV, RG, SET>);                \
+        MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV, RG, SET>);                            \
+        MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV, RG, SET>);                             \
     } while (0)
-    if (bf16 && gwords == Payload<Bf16x4G32>::kWords) MVP_LAUNCH_BWD_T(Bf16x4G32);
-    else if (bf16) MVP_LAUNCH_BWD_T(Bf16x4);
-    else MVP_LAUNCH_BWD_T(float4);
+#define MVP_LAUNCH_BWD_ANY(TT, WW_, VV)                                                                      \
+    do {                                                                                                     \
+        if (set == kGradRaysOnly) MVP_LAUNCH_BWD_SET(TT, WW_, VV, true, kGradRaysOnly);                      \
+        else if (set == kGradNoPayload && rays) MVP_LAUNCH_BWD_SET(TT, WW_, VV, true, kGradNoPayload);       \
+        else if (set == kGradNoPayload) MVP_LAUNCH_BWD_SET(TT, WW_, VV, false, kGradNoPayload);              \
+        else MVP_LAUNCH_BWD(TT, WW_, VV);                                                                    \
+    } while (0)
+#define MVP_LAUNCH_BWD_T(LAUNCH, VV)                                                             \
+    do {                                                                                         \
+        if (a->algo == 1) LAUNCH(0, true, VV);                                                   \
+        else if (cubic == 8) LAUNCH(8, false, VV);                                               \
+        else if (cubic == 16) LAUNCH(16, false, VV);                                             \
+        else LAUNCH(0, false, VV);                                                               \
+    } while (0)
+    if (bf16 && gwords == Payload<Bf16x4G32>::kWords && set == kGradAll) MVP_LAUNCH_BWD_T(MVP_LAUNCH_BWD, Bf16x4G32);
+    else if (bf16) MVP_LAUNCH_BWD_T(MVP_LAUNCH_BWD_ANY, Bf16x4);
+    else MVP_LAUNCH_BWD_T(MVP_LAUNCH_BWD_ANY, float4);
 #undef MVP_LAUNCH_BWD_T
+#undef MVP_LAUNCH_BWD_ANY
+#undef MVP_LAUNCH_BWD_SET
 #undef MVP_LAUNCH_BWD
     cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? MVP_OK : (int)e;

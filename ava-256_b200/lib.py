@@ -73,6 +73,8 @@ FLAG_ZERO_GRADS = 2
 FLAG_SHARED_PRIMS = 4
 FLAG_TPLATE_BF16 = 8
 FLAG_GRAD_TPLATE_F32 = 16
+FLAG_NO_TPLATE_GRAD = 32
+FLAG_RAY_GRADS_ONLY = 64
 FLAG_TEST_TINY_LISTS = 0x100
 ABI_VERSION = 8
 # layout pins, equal to the static_asserts in csrc/mvp_kernels.cu (tests/test_abi.py compares)
@@ -195,6 +197,13 @@ def require_ray_grads():
     mvp_compute_raydirs_backward), which it reports as RAY_GRADS=1 in its build configuration."""
     if "RAY_GRADS=1" not in LIB.mvp_build_config().decode().split():
         raise RuntimeError("mvpraymarch_b200: this library (%s) does not support gradients of rays and cameras" % _build.LIB)
+
+
+def require_grad_select():
+    """Raise unless the library computes reduced gradient sets (MVP_FLAG_NO_TPLATE_GRAD, MVP_FLAG_RAY_GRADS_ONLY), which it reports
+    as GRAD_SELECT=1 in its build configuration.  An older library ignores the two bits and would write to NULL buffers."""
+    if "GRAD_SELECT=1" not in LIB.mvp_build_config().decode().split():
+        raise RuntimeError("mvpraymarch_b200: this library (%s) does not support reduced gradient sets" % _build.LIB)
 
 
 def workspace_bytes(N, H, W, K, TD, TH, TW):

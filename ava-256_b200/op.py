@@ -96,6 +96,32 @@ def _empty_template_grad(template, tflags):
     return torch.empty_like(template)
 
 
+# Gradient sets of the backward, chosen by the forward from what autograd asks for (ctx.needs_input_grad):
+#   GRADS_ALL         transforms, template (+ warp), optionally rays: the template or the warp needs a gradient
+#   GRADS_NO_PAYLOAD  transforms, optionally rays (MVP_FLAG_NO_TPLATE_GRAD): no payload-gradient scatter, no template-sized buffer
+#   GRADS_RAYS_ONLY   rays only (MVP_FLAG_RAY_GRADS_ONLY): a frozen avatar seen through a differentiable camera
+GRADS_ALL, GRADS_NO_PAYLOAD, GRADS_RAYS_ONLY = "all", "no_payload", "rays_only"
+_GRAD_SET_FLAGS = {GRADS_ALL: 0, GRADS_NO_PAYLOAD: _lib.FLAG_NO_TPLATE_GRAD, GRADS_RAYS_ONLY: _lib.FLAG_RAY_GRADS_ONLY}
+
+
+def _grad_set(needs, first_prim, want_rays):
+    """The gradient set for ctx.needs_input_grad `needs` whose primitive inputs (primpos, primrot, primscale, template, warp) start
+    at index first_prim; None when nothing needs a gradient."""
+    if needs[first_prim + 3] or needs[first_prim + 4]:
+        return GRADS_ALL
+    if any(needs[first_prim:first_prim + 3]):
+        return GRADS_NO_PAYLOAD
+    return GRADS_RAYS_ONLY if want_rays else None
+
+
+def _empty_grads(gset, primpos, primrot, primscale, template, warp, usewarp, tflags):
+    """The backward's gradient buffers of the set: [primpos, primrot, primscale, template, warp], None where not computed."""
+    tf = [torch.empty_like(primpos), torch.empty_like(primrot), torch.empty_like(primscale)] if gset != GRADS_RAYS_ONLY else [None] * 3
+    if gset != GRADS_ALL:
+        return tf + [None, None]
+    return tf + [_empty_template_grad(template, tflags), torch.empty_like(warp) if usewarp else None]
+
+
 class MVPRaymarch(Function):
     """Custom Function for raymarching Mixture of Volumetric Primitives (reference: mvpraymarch.py:87-292)."""
 
@@ -107,8 +133,10 @@ class MVPRaymarch(Function):
 
     @staticmethod
     def _forward(ctx, raypos, raydir, stepsize, tminmax, primpos, primrot, primscale, template, warp, rayterm,
-                 gradmode, options, saved_extra=()):
-        """The forward; saved_extra: more tensors for ctx.save_for_backward, after the eleven the backward reads."""
+                 gradmode, options, saved_extra=(), first_prim=4, ray_inputs=(0, 1, 3)):
+        """The forward; saved_extra: more tensors for ctx.save_for_backward, after the eleven the backward reads.  first_prim: index
+        of primpos among the Function's inputs (primrot, primscale, template and warp follow); ray_inputs: the inputs through which
+        the rays get gradients (with the `_ray_grads` option).  They pick the backward's gradient set from ctx.needs_input_grad."""
         algo = options["algo"]
         if algo not in (0, 1):
             raise NotImplementedError("mvpraymarch_b200: algo must be 0 or 1 (the reference launches nothing for other "
@@ -143,7 +171,18 @@ class MVPRaymarch(Function):
                 _check_f32_cuda(name, t)
         _check_f32_cuda("template", template, allow_bf16=True)
         bf16 = template.dtype == torch.bfloat16                        # MVP_FLAG_TPLATE_BF16: rendered as template.float()
-        grad_f32 = bf16 and _check_template_grad_dtype(options.get("_template_grad_dtype")) is torch.float32
+        gset = None
+        if gradmode:
+            # Only the gradients autograd asks for.  With none that this op computes, the image is rendered as in inference.  The
+            # output may still get a backward (rays that require grad without the `_ray_grads` option: they get None, as before),
+            # which then returns None for every input: ctx.gset = None.
+            needs = ctx.needs_input_grad
+            gset = _grad_set(needs, first_prim, bool(options.get("_ray_grads")) and any(needs[i] for i in ray_inputs))
+            gradmode = gset is not None
+            ctx.gset = gset
+            if gset not in (None, GRADS_ALL):
+                _lib.require_grad_select()
+        grad_f32 = bf16 and _check_template_grad_dtype(options.get("_template_grad_dtype")) is torch.float32 and gset == GRADS_ALL
         tflags = _lib.tplate_flags(bf16, grad_f32)                     # + MVP_FLAG_GRAD_TPLATE_F32: fp32 template gradient
         if warp is not None:                                           # mvpraymarch.py:124
             assert warp.is_contiguous() and warp.dim() == 6 and warp.size(-1) == 3, \
@@ -190,7 +229,7 @@ class MVPRaymarch(Function):
             a = _lib.ForwardArgs()
             a.shape = _lib.Shape(N, H, W, K, TD, TH, TW)
             a.stepsize, a.fadescale, a.fadeexp = float(stepsize), float(options["fadescale"]), float(options["fadeexp"])
-            a.flags = (_lib.FLAG_SHARED_PRIMS if shared else 0) | tflags
+            a.flags = (_lib.FLAG_SHARED_PRIMS if shared else 0) | tflags | _GRAD_SET_FLAGS.get(gset, 0)
             a.raypos, a.raydir, a.tminmax = _ptr(raypos), _ptr(raydir), _ptr(tminmax)
             if camera is not None:
                 a.camera = _lib.Camera(_ptr(viewpos), _ptr(viewrot), _ptr(focal), _ptr(princpt), float(volradius), 0)
@@ -211,9 +250,9 @@ class MVPRaymarch(Function):
             grads = None
             if gradmode:
                 # The gradient buffers of the backward (mvpraymarch.py:240-246 zeros_like's them there) are made now and zero-filled
-                # by the forward's render kernel on the side (mvp_forward_args::clear_grad_*): no memset pass in the step.
-                grads = [torch.empty_like(primpos), torch.empty_like(primrot), torch.empty_like(primscale),
-                         _empty_template_grad(template, tflags), torch.empty_like(warp) if usewarp else None]
+                # by the forward's render kernel on the side (mvp_forward_args::clear_grad_*): no memset pass in the step.  Only
+                # those of the gradient set: a frozen template costs no template-sized buffer.
+                grads = _empty_grads(gset, primpos, primrot, primscale, template, warp, usewarp, tflags)
                 a.clear_grad_primpos, a.clear_grad_primrot, a.clear_grad_primscale = _ptr(grads[0]), _ptr(grads[1]), _ptr(grads[2])
                 a.clear_grad_tplate, a.clear_grad_warp = _ptr(grads[3]), _ptr(grads[4])
             stream = torch.cuda.current_stream(dev).cuda_stream
@@ -238,6 +277,8 @@ class MVPRaymarch(Function):
     def backward(ctx, grad_rayrgba, grad_rayalpha=None):
         """grad_rayrgba [N,H,W,4]; or, for MVPRaymarchPlanes, (grad_rayrgb [N,3,H,W], grad_rayalpha [N,1,H,W]).  With the
         `_ray_grads` option (a differentiable `compute_raydirs` feeds the rays, see `mvpraymarch_camera`) the rays get gradients too."""
+        if ctx.gset is None:                   # no input of this op gets a gradient (see _forward): nothing to compute
+            return (None,) * 12
         want_rays = bool(ctx.options.get("_ray_grads")) and any(ctx.needs_input_grad[i] for i in (0, 1, 3))
         prim, rays = _march_backward(ctx, grad_rayrgba, grad_rayalpha, want_rays)
         grad_raypos, grad_raydir, grad_tminmax = rays if rays is not None else (None, None, None)
@@ -246,7 +287,8 @@ class MVPRaymarch(Function):
 
 def _march_backward(ctx, grad_rayrgba, grad_rayalpha, want_rays):
     """The native backward of an MVPRaymarch forward: ((grad_primpos, grad_primrot, grad_primscale, grad_template, grad_warp),
-    (grad_raypos, grad_raydir, grad_tminmax) with want_rays (mvp_raymarch_backward_rays), else None)."""
+    (grad_raypos, grad_raydir, grad_tminmax) with want_rays (mvp_raymarch_backward_rays), else None).  The primitive gradients
+    outside the forward's gradient set (ctx.gset) are None."""
     raypos, raydir, tminmax, primpos, primrot, primscale, template, raysat, rayaux, workspace, warp = ctx.saved_tensors[:11]
     options = ctx.options
     N, H, W = ctx.nhw
@@ -262,19 +304,21 @@ def _march_backward(ctx, grad_rayrgba, grad_rayalpha, want_rays):
         else:
             grad_rayrgba = _aligned(grad_rayrgba.contiguous(), 16)     # mvpraymarch.py:264
         usewarp = options["algo"] == 1
+        gset = ctx.gset
+        if gset == GRADS_RAYS_ONLY:
+            assert want_rays, "a rays-only backward without ray gradients"
         grads, ctx.grads = ctx.grads, None
         fresh = grads is not None          # the forward's render kernel zero-filled them; a second backward through the
         if not fresh:                      # same graph (retain_graph) gets new ones, zero-filled by the library
-            grads = [torch.empty_like(primpos), torch.empty_like(primrot), torch.empty_like(primscale),
-                     _empty_template_grad(template, ctx.tflags), torch.empty_like(warp) if usewarp else None]
+            grads = _empty_grads(gset, primpos, primrot, primscale, template, warp, usewarp, ctx.tflags)
         grad_primpos, grad_primrot, grad_primscale, grad_template, grad_warp = grads
-        if warp is not None and not usewarp:                       # mvpraymarch.py:246 (zero when algo 0 ignores it)
+        if warp is not None and not usewarp and gset == GRADS_ALL:  # mvpraymarch.py:246 (zero when algo 0 ignores it)
             grad_warp = torch.zeros_like(warp)
         a = _lib.BackwardArgs()
         a.shape = _lib.Shape(N, H, W, K, TD, TH, TW)
         a.stepsize, a.fadescale, a.fadeexp = ctx.stepsize, float(options["fadescale"]), float(options["fadeexp"])
         a.flags = _lib.FLAG_ACCEL_VALID | (0 if fresh else _lib.FLAG_ZERO_GRADS) | (_lib.FLAG_SHARED_PRIMS if ctx.shared else 0) | \
-            ctx.tflags
+            ctx.tflags | _GRAD_SET_FLAGS[gset]
         a.raypos, a.raydir, a.tminmax = _ptr(raypos), _ptr(raydir), _ptr(tminmax)
         if ctx.camera is not None:
             viewpos, viewrot, focal, princpt, volradius = ctx.camera[:5]
@@ -331,10 +375,12 @@ class MVPRaymarchCameraGrad(Function):
     def forward(ctx, viewpos, viewrot, focal, princpt, stepsize, primpos, primrot, primscale, template, warp, gradmode, options):
         # the camera tensors are saved for backward: the adjoint recomputes the rays from them
         return MVPRaymarch._forward(ctx, None, None, stepsize, None, primpos, primrot, primscale, template, warp, None, gradmode, options,
-                                    saved_extra=(viewpos, viewrot, focal, princpt))
+                                    saved_extra=(viewpos, viewrot, focal, princpt), first_prim=5, ray_inputs=(0, 1, 2, 3))
 
     @staticmethod
     def backward(ctx, grad_out, grad_rayalpha=None):
+        if ctx.gset is None:
+            return (None,) * 12
         prim, rays = _march_backward(ctx, grad_out, grad_rayalpha, True)
         viewpos, viewrot, focal, princpt = ctx.saved_tensors[11:15]
         volradius = ctx.camera[4]
@@ -492,7 +538,8 @@ def mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, volradius,
     utils.py:45-46).  With camera_grad=True, viewpos, viewrot, focal and princpt are autograd inputs and those that require grad get
     the gradient of the image with every discrete decision of the march held fixed (C-ABI mvp_raymarch_backward_rays, then the ray
     generator's adjoint mvp_compute_raydirs_backward); pixelcoords and volradius get none.  When no camera tensor requires grad,
-    the plain backward runs.
+    the plain backward runs.  The backward computes only what requires grad: with the template and transforms detached (a frozen
+    avatar) it computes the ray gradients alone, with no template-sized gradient buffer and no payload-gradient scatter.
     template_grad_dtype=torch.float32 accumulates a bfloat16 template's gradient in fp32 (see the `template_grad_dtype` context
     manager); None leaves the setting of an enclosing `template_grad_dtype` block, by default the template's own dtype.
     Returns rayrgba [N,H,W,4], or (rayrgb [N,3,H,W], rayalpha [N,1,H,W]) with planes=True."""

@@ -92,6 +92,18 @@ typedef struct mvp_shape {
                                  * Like MVP_FLAG_TPLATE_BF16 it must be the same in a forward and the backward that follows it: the
                                  * forward sizes its clear of clear_grad_tplate by it.  The library supports it iff
                                  * mvp_build_config() lists GRAD_TPLATE_F32=1 (an older one ignores the bit). */
+#define MVP_FLAG_NO_TPLATE_GRAD 32u /* forward and backward: no gradient of the template or the warp field is wanted.  grad_tplate,
+                                 * grad_warp, clear_grad_tplate and clear_grad_warp may then be NULL, and are neither read nor
+                                 * written if they are not.  The backward computes the transform gradients (and with
+                                 * mvp_raymarch_backward_rays the ray gradients) without the payload-gradient scatter, its most
+                                 * expensive part; they equal those of the full backward up to the order of the fp32 atomics.
+                                 * MVP_FLAG_GRAD_TPLATE_F32 has no effect with it.  Without this flag or the next one a NULL gradient
+                                 * pointer is MVP_ERR_NULL.  The library supports it iff mvp_build_config() lists GRAD_SELECT=1. */
+#define MVP_FLAG_RAY_GRADS_ONLY 64u /* forward and mvp_raymarch_backward_rays: only the ray gradients are wanted.  The rule above
+                                 * extends to every primitive gradient (grad_primpos / primrot / primscale / tplate / warp and every
+                                 * clear_grad_*): they may be NULL and are ignored.  The backward skips the payload scatter and the
+                                 * transform-gradient sums.  mvp_raymarch_backward with this flag returns MVP_ERR_NULL: it would have
+                                 * no output.  MVP_FLAG_ZERO_GRADS zero-fills only the buffers a call's flags request. */
 #define MVP_FLAG_TEST_TINY_LISTS 0x100u /* test hook: forward keeps at most 16 saved tile-list entries per view, so almost
                                  * every tile takes the backward's rebuild path */
 
