@@ -906,6 +906,30 @@ __device__ __forceinline__ bool slab_test_margin(const Prim &q, const Ray &r, fl
     him = fminf(fminf(x0 + w0, x1 + w1), x2 + w2);
     return lo <= hi;
 }
+
+// The two margins of a ray's step intervals, shared by the tile lists (build_tile_list) and the backward's per-slab intervals so
+// that both see the same samples:
+//   epos (world units) bounds |computed position at step j - exact point o + (tmin + j dt) d| over every step of the ray, plus
+//     the rounding of the slab tests.  The march rounds each component once per step (x = fma(d, dt, x)), three more times at
+//     the start; while |x_i| <= X a rounding is at most X 2^-24 (half an ulp), and sqrt(3) takes the three components to a norm.
+//     The rounding is not random: in one binade every step can round the same way, so the drift does reach this bound.  X is
+//     the march's largest coordinate, at least 2: the segment from o + tmin d to o + tmax d, on which every position lies, is
+//     convex, so its end points bound it.  On top, 16 X 2^-24 covers the rounding inside the slab transform and the inside
+//     test, relative to the coordinates the march reaches, and |o| 2^-22 the rounding of the slab test's o - p, which is
+//     relative to the ray's origin.  For X <= 2 and |o| <= 8 (every ray that starts outside the unit cube at a camera distance
+//     of up to 8 and marches inside it) epos is the float it was when the bound assumed |x| < 2.
+//   eps0 (steps) covers the rounding of the t -> step conversion, relative to the larger of the ray's step count and the
+//     lattice origin tmin / dt.
+// A non-finite end point or tmax makes epos infinite, which only widens the intervals to every step.
+__device__ __forceinline__ void march_margins(const Ray &r, float rdt, float &epos, float &eps0) {
+    const float nsteps = fmaxf(r.tmax - r.tmin, 0.f) * rdt + 8.f;
+    const float a = fmaxf(fmaxf(fabsf(__fmaf_rn(r.dx, r.tmin, r.ox)), fabsf(__fmaf_rn(r.dy, r.tmin, r.oy))), fabsf(__fmaf_rn(r.dz, r.tmin, r.oz)));
+    const float b = fmaxf(fmaxf(fabsf(__fmaf_rn(r.dx, r.tmax, r.ox)), fabsf(__fmaf_rn(r.dy, r.tmax, r.oy))), fabsf(__fmaf_rn(r.dz, r.tmax, r.oz)));
+    const float u = fmaxf(2.f, fmaxf(a, b)) * 5.9604645e-8f;                      // X 2^-24 (fmaxf drops a NaN end point)
+    const float o = fmaxf(fmaxf(fabsf(r.ox), fabsf(r.oy)), fabsf(r.oz));
+    epos = 1.7320508f * nsteps * u + fmaxf(16.f * u, o * 2.3841858e-7f);
+    eps0 = fmaxf(0.001953125f, (nsteps + fabsf(r.tmin * rdt)) * 4.7683716e-7f);
+}
 #endif
 
 __device__ __forceinline__ int clamp_step(float v) {   // float -> step index, saturating, NaN -> +big
@@ -1106,12 +1130,8 @@ __device__ __forceinline__ bool build_tile_list(const Params &p, float rdt, int 
     c.off = clamp_step(ceilf(tref - tsteps));
     const float foff = (float)c.off;
 #if MVP_LIST_MARGIN
-    // Bound on |computed position at step j - exact point o + (tmin + j dt) d| for every step of this ray: one rounding of at
-    // most 2^-23 per component and step (|x| < 2), three more at the start, sqrt(3) for the norm; 2^-19 on top covers
-    // the rounding inside the slab transform and the slab test themselves.  In steps: see eps0.
-    const float nsteps = fmaxf(c.ray.tmax - c.ray.tmin, 0.f) * rdt + 8.f;
-    const float epos = 1.7320508f * nsteps * 1.1920929e-7f + 1.9073486e-6f;
-    const float eps0 = fmaxf(0.001953125f, nsteps * 4.7683716e-7f);
+    float epos, eps0;                                 // drift bound of this ray's marched positions, see march_margins
+    march_margins(c.ray, rdt, epos, eps0);
 #endif
 
     const float4 *packn = p.pack + (size_t)(n * p.pview) * p.K * 4;
@@ -2175,10 +2195,8 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                 {
                     Ray ry;
                     ry.ox = L_OX; ry.oy = L_OY; ry.oz = L_OZ; ry.dx = rdx; ry.dy = rdy; ry.dz = rdz; ry.tmin = L_TMIN; ry.tmax = L_TMAX;
-                    const float nsteps = fmaxf(ry.tmax - ry.tmin, 0.f) * rdt + 8.f;
-                    const float epos = 1.7320508f * nsteps * 1.1920929e-7f + 1.9073486e-6f;
-                    const float eps0 = fmaxf(0.001953125f, nsteps * 4.7683716e-7f);
-                    float lom, him;
+                    float epos, eps0, lom, him;
+                    march_margins(ry, rdt, epos, eps0);
                     slab_test_margin(q, ry, epos, lo, hi, lom, him);
                     if (hashit && lom <= him) {
                         la = max(clamp_step(ceilf((lom - ry.tmin) * rdt - eps0) - foff), max(L_MS, cs));
