@@ -421,21 +421,58 @@ __global__ void __launch_bounds__(128) cam_params_kernel(int N, const float *__r
 // 2. per-slab record + pixel rectangle
 //    record (4 x float4): (pos.xyz, s.x) (R row0, s.y) (R row1, s.z) (R row2, 0)
 // ------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) prim_setup_kernel(int N, int K, int H, int W, int pview, const float *__restrict__ primpos,
+// The primitive set of view n in a sets call (mvp_raymarch_forward_sets): view_set[n], which comes from outside the program.  An
+// entry outside [0, nsets) reads as set 0, so that no address derived from it leaves the tensors; prim_setup_kernel gives such a
+// view empty rectangles, so nothing of set 0 is ever sampled for it and it renders empty.
+__device__ __forceinline__ int checked_set(const int *__restrict__ vset, int nsets, int n) {
+    const unsigned s = (unsigned)__ldg(vset + n);
+    return s < (unsigned)nsets ? (int)s : 0;
+}
+
+// The marching order of view n's primitives: one per view (ostride K), one shared by all views (ostride 0), or its set's
+__device__ __forceinline__ const int *view_order(const int *order, int n, int ostride, const int *vset, int nsets, int K) {
+    if (!order) return nullptr;
+    return vset ? order + (size_t)checked_set(vset, nsets, n) * K : order + (size_t)n * ostride;
+}
+
+__device__ __forceinline__ void store_record(float4 *__restrict__ pack, size_t ip, const float *pp, const float *r, const float *ps) {
+    pack[ip * 4 + 0] = make_float4(pp[0], pp[1], pp[2], ps[0]);
+    pack[ip * 4 + 1] = make_float4(r[0], r[1], r[2], ps[1]);
+    pack[ip * 4 + 2] = make_float4(r[3], r[4], r[5], ps[2]);
+    pack[ip * 4 + 3] = make_float4(r[6], r[7], r[8], 0.f);
+}
+
+// vset (sets calls, else NULL): thread i also writes record i of the nsets * K records -- every set's records once, whichever
+// views reference it -- and the rectangle of slab i % K in view i / K from the primitives of that view's set.
+__global__ void __launch_bounds__(128) prim_setup_kernel(int N, int K, int H, int W, int pview, const int *__restrict__ vset, int nsets,
+                                                         const float *__restrict__ primpos,
                                                          const float *__restrict__ primrot, const float *__restrict__ primscale,
                                                          const Cam *__restrict__ cam, const int *__restrict__ bad,
                                                          float4 *__restrict__ pack, unsigned *__restrict__ rx, unsigned *__restrict__ ry) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (size_t)N * K) return;
     const int n = (int)(i / (size_t)K);
-    const size_t ip = pview ? i : i - (size_t)n * K;     // index of the slab in the primitive tensors / record array
+    size_t ip = pview ? i : i - (size_t)n * K;           // index of the slab in the primitive tensors / record array
+    bool own_record = pview || n == 0;
+    if (vset) {
+        if (i < (size_t)nsets * K) {
+            float rr[9];
+#pragma unroll
+            for (int j = 0; j < 9; ++j) rr[j] = primrot[i * 9 + j];
+            store_record(pack, i, primpos + i * 3, rr, primscale + i * 3);
+        }
+        const unsigned s = (unsigned)__ldg(vset + n);
+        if (s >= (unsigned)nsets) { rx[i] = 1u; ry[i] = 1u; return; }   // (1, 0): empty -- no tile of the view lists a slab
+        ip = (size_t)s * K + (i - (size_t)n * K);
+        own_record = false;
+    }
     const float *pp = primpos + ip * 3, *pr = primrot + ip * 9, *ps = primscale + ip * 3;
     float p0 = pp[0], p1 = pp[1], p2 = pp[2];
     float r[9];
 #pragma unroll
     for (int j = 0; j < 9; ++j) r[j] = pr[j];
     float s0 = ps[0], s1 = ps[1], s2 = ps[2];
-    if (pview || n == 0) {
+    if (own_record) {
         pack[ip * 4 + 0] = make_float4(p0, p1, p2, s0);
         pack[ip * 4 + 1] = make_float4(r[0], r[1], r[2], s1);
         pack[ip * 4 + 2] = make_float4(r[3], r[4], r[5], s2);
@@ -485,7 +522,8 @@ __global__ void __launch_bounds__(128) prim_setup_kernel(int N, int K, int H, in
 // y range (pixels) of every block of 32 slabs consecutive in DFS rank: the bucket kernels test a block before its slabs, so a
 // tile row only touches the ~10-20 % of the blocks that can reach it (slabs follow the UV grid: consecutive ranks are neighbours).
 __global__ void __launch_bounds__(256) block_ranges_kernel(int K, const unsigned *__restrict__ ry, const int *__restrict__ order,
-                                                           int ostride, unsigned *__restrict__ blky) {
+                                                           int ostride, const int *__restrict__ vset, int nsets,
+                                                           unsigned *__restrict__ blky) {
     const int lane = threadIdx.x & 31;
     const int NB = (K + 31) / 32;
     const int blk = blockIdx.x * 8 + (threadIdx.x >> 5), n = blockIdx.y;
@@ -494,7 +532,7 @@ __global__ void __launch_bounds__(256) block_ranges_kernel(int K, const unsigned
     const int j = blk * 32 + lane;
     int y0 = 0xffff, y1 = -1;
     if (j < K) {
-        const int k = slab_at_rank(order ? order + (size_t)n * ostride : nullptr, K, kstart, j);
+        const int k = slab_at_rank(view_order(order, n, ostride, vset, nsets, K), K, kstart, j);
         const unsigned yr = __ldg(ry + (size_t)n * K + k);
         const int a = (int)(yr & 0xffffu), b = (int)(yr >> 16);
         if (a <= b) { y0 = a; y1 = b; }
@@ -512,6 +550,7 @@ constexpr int kRowThreads = 256;          // 8 warps = 8 tile rows per CTA
 __global__ void __launch_bounds__(kRowThreads) row_lists_kernel(int K, int R, int rowcap, int TXn,
                                                                 const unsigned *__restrict__ rx, const unsigned *__restrict__ ry,
                                                                 const unsigned *__restrict__ blky, const int *__restrict__ order, int ostride,
+                                                                const int *__restrict__ vset, int nsets,
                                                                 int *__restrict__ rowcnt, RowEntry *__restrict__ rowlist
 #if MVP_XBUCKETS
                                                                 , int NG, int2 *__restrict__ grphdr, RowEntry *__restrict__ grplist,
@@ -525,7 +564,7 @@ __global__ void __launch_bounds__(kRowThreads) row_lists_kernel(int K, int R, in
     const unsigned *rxn = rx + (size_t)n * K, *ryn = ry + (size_t)n * K;
     RowEntry *out = rowlist + ((size_t)n * R + row) * rowcap;
     const int kstart = dfs_kstart(K);
-    const int *ordn = order ? order + (size_t)n * ostride : nullptr;
+    const int *ordn = view_order(order, n, ostride, vset, nsets, K);
     const unsigned below = (1u << lane) - 1u;
     int total = 0;
     const int NB = (K + 31) / 32;
@@ -618,6 +657,7 @@ __global__ void __launch_bounds__(kRowThreads) row_lists_kernel(int K, int R, in
 __global__ void __launch_bounds__(kRowThreads) row_lists_cta_kernel(int K, int R, int rowcap, int TXn,
                                                                     const unsigned *__restrict__ rx, const unsigned *__restrict__ ry,
                                                                     const unsigned *__restrict__ blky, const int *__restrict__ order, int ostride,
+                                                                    const int *__restrict__ vset, int nsets,
                                                                     int *__restrict__ rowcnt, RowEntry *__restrict__ rowlist
 #if MVP_XBUCKETS
                                                                     , int NG, int2 *__restrict__ grphdr, RowEntry *__restrict__ grplist,
@@ -631,7 +671,7 @@ __global__ void __launch_bounds__(kRowThreads) row_lists_cta_kernel(int K, int R
     const unsigned *rxn = rx + (size_t)n * K, *ryn = ry + (size_t)n * K;
     RowEntry *out = rowlist + ((size_t)n * R + row) * rowcap;
     const int kstart = dfs_kstart(K);
-    const int *ordn = order ? order + (size_t)n * ostride : nullptr;
+    const int *ordn = view_order(order, n, ostride, vset, nsets, K);
     const unsigned below = (1u << lane) - 1u;
     __shared__ int s_cnt[NW];
     // the warp's segment of the rank-ordered sequence, in blocks of 32 slabs; only blocks whose y range reaches the row are read
@@ -1083,7 +1123,17 @@ struct Params {
     // appended last so that the parameter offsets of every other kernel stay what they were)
     float *g_raypos, *g_raydir;
     float2 *g_tminmax;
+    // sets calls (kSets kernels only): view n renders primitive set vset[n] of nsets, see checked_set
+    const int *vset;
+    int nsets;
 };
+
+// Index of view n's primitive set: n (per-view tensors), 0 (MVP_FLAG_SHARED_PRIMS) or, in the kSets kernels, its checked map entry
+template <bool kSets>
+__device__ __forceinline__ int prim_set(const Params &p, int n) {
+    if (kSets) return checked_set(p.vset, p.nsets, n);
+    return n * p.pview;
+}
 
 #if defined(MVP_CPU_EMUL) && defined(MVP_EMUL_STATS)
 long long g_emul_list_chunks;   // 32-entry bucket chunks scanned by build_tile_list (forward + backward)
@@ -1112,7 +1162,7 @@ __device__ __forceinline__ bool tile_bucket_empty(const Params &p, int n, int tx
 // "every lane starts at its own first hit" (the reference's lock-step loop) and over a plane fitted to the first-hit
 // depths because neighbouring slabs sit at randomly different depths while the sweep planes stay coherent.
 // Returns false when the list would exceed CAP (< 512): the caller hands the tile to the 512-entry kernel.
-template <int CAP, bool kPrefetch>
+template <int CAP, bool kPrefetch, bool kSets>
 __device__ __forceinline__ bool build_tile_list(const Params &p, float rdt, int n, int tx, int ty, int lane, TileCtx &c,
                                                 int *s_k, int *s_iv, RowEntry *s_stage, unsigned long long *s_bar, float &t,
                                                 float &x, float &y, float &z, float &r1e, int &j0) {
@@ -1134,7 +1184,7 @@ __device__ __forceinline__ bool build_tile_list(const Params &p, float rdt, int 
     march_margins(c.ray, rdt, epos, eps0);
 #endif
 
-    const float4 *packn = p.pack + (size_t)(n * p.pview) * p.K * 4;
+    const float4 *packn = p.pack + (size_t)prim_set<kSets>(p, n) * p.K * 4;
     const int cnt = p.rowcnt[(size_t)n * p.R + ty];
     const bool overflow = cnt > p.rowcap;
 #if MVP_XBUCKETS
@@ -1184,7 +1234,7 @@ __device__ __forceinline__ bool build_tile_list(const Params &p, float rdt, int 
                 k = e.k; xr = e.xr;
                 cand = true;
             } else {
-                k = slab_at_rank(p.order ? p.order + (size_t)(n * p.pview) * p.K : nullptr, p.K, kstart, idx);
+                k = slab_at_rank(p.order ? p.order + (size_t)prim_set<kSets>(p, n) * p.K : nullptr, p.K, kstart, idx);
                 xr = __ldg(rxn + k);
                 unsigned yr = __ldg(ryn + k);
                 int y0 = (int)(yr & 0xffffu), y1 = (int)(yr >> 16);
@@ -1252,7 +1302,7 @@ __device__ __forceinline__ bool build_tile_list(const Params &p, float rdt, int 
     // TMA bulk prefetch (cp.async.bulk.prefetch.L2): pull the payload slabs this tile is about to sample into L2 while
     // the lattice set-up runs; one lane per slab, fire and forget.
     if (kPrefetch && p.slab_bytes >= 16) {
-        const char *tp = reinterpret_cast<const char *>(p.tplate) + (size_t)(n * p.pview) * p.K * p.slab_bytes;
+        const char *tp = reinterpret_cast<const char *>(p.tplate) + (size_t)prim_set<kSets>(p, n) * p.K * p.slab_bytes;
         for (int i = lane; i < nl; i += 32) {
             const char *a = tp + (size_t)s_k[i] * p.slab_bytes;
             asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(a), "r"(p.slab_bytes) : "memory");
@@ -1558,7 +1608,7 @@ struct __align__(16) FwdWarpSmem {   // per-warp shared state of the forward ker
 //    fits (almost all) with a small shared-memory footprint (more L1 for the voxel gathers) and flags the rest;
 //    the CAP == 512 variant then renders only the flagged tiles.
 // ------------------------------------------------------------------------------------------------------
-template <int T, bool kGrad, int CAP, bool kWarp, typename V>
+template <int T, bool kGrad, int CAP, bool kWarp, typename V, bool kSets>
 __device__ __forceinline__ bool forward_tile(const Params &p, const int n, const int tx, const int ty, const int lane, FwdWarpSmem<CAP, kGrad> *const S) {
     // all per-warp shared state lives in one record: every address below is (one pinned per-warp base) + immediate
     int *const sk = S->k, *const siv = S->iv, *const rm = S->rm;
@@ -1597,7 +1647,7 @@ __device__ __forceinline__ bool forward_tile(const Params &p, const int n, const
     TileCtx c;
     float t, x, y, z, r1e;
     int j0;
-    if (!build_tile_list<CAP, true>(p, rdt, n, tx, ty, lane, c, sk, siv, sstage, sbar, t, x, y, z, r1e, j0)) return false;
+    if (!build_tile_list<CAP, true, kSets>(p, rdt, n, tx, ty, lane, c, sk, siv, sstage, sbar, t, x, y, z, r1e, j0)) return false;
 
     const int px = tx * kTileW + (lane & 7), py = ty * kTileH + (lane >> 3);
     const size_t r = ((size_t)n * p.H + min(py, p.H - 1)) * p.W + min(px, p.W - 1);
@@ -1625,11 +1675,11 @@ __device__ __forceinline__ bool forward_tile(const Params &p, const int n, const
     if (nl > 192) MVP_STAT2(7, 1);
 #endif
     const int nwords = (nl + 31) >> 5;
-    const float4 *packn = p.pack + (size_t)(n * p.pview) * p.K * 4;
+    const float4 *packn = p.pack + (size_t)prim_set<kSets>(p, n) * p.K * 4;
     // voxels per slab: a compile-time constant for the cubic 8^3 / 16^3 specialisations, so that a slab's address is a shift and an add
     // wherever the register cap makes the compiler re-derive it (it was ~30 of the 159 instructions of a batch gather)
     const size_t slabsz = T > 0 ? (size_t)(T * T * T) : (size_t)p.TD * p.TH * p.TW;
-    const V *tpn = reinterpret_cast<const V *>(p.tplate) + (size_t)(n * p.pview) * p.K * slabsz;
+    const V *tpn = reinterpret_cast<const V *>(p.tplate) + (size_t)prim_set<kSets>(p, n) * p.K * slabsz;
     const int kstart = dfs_kstart(p.K);
     {
         // pinned: under the register cap the compiler would otherwise re-materialise this base address per event
@@ -1667,7 +1717,7 @@ __device__ __forceinline__ bool forward_tile(const Params &p, const int n, const
                     sat = true;
                     if (kGrad) {
                         jsat = rm[b] + c.off;
-                        ranksat = rank_of_slab(p.rankof ? p.rankof + (size_t)(n * p.pview) * p.K : nullptr, p.K, kstart, sk[(__float_as_int(rr.w) >> 5) & 1023]);
+                        ranksat = rank_of_slab(p.rankof ? p.rankof + (size_t)prim_set<kSets>(p, n) * p.K : nullptr, p.K, kstart, sk[(__float_as_int(rr.w) >> 5) & 1023]);
                         abefore = acc.w;
                     }
                 }
@@ -1683,7 +1733,7 @@ __device__ __forceinline__ bool forward_tile(const Params &p, const int n, const
         float4 sres = make_float4(0.f, 0.f, 0.f, 0.f);
         if (act) {
             const int kk = sk[(__float_as_int(rec.w) >> 5) & 1023];
-            if (kWarp) sres = sample_slab_warped(tpn + (size_t)kk * slabsz, p.warp + ((size_t)(n * p.pview) * p.K + kk) * ((size_t)p.WD * p.WH * p.WW * 3), rec.x, rec.y, rec.z, p);
+            if (kWarp) sres = sample_slab_warped(tpn + (size_t)kk * slabsz, p.warp + ((size_t)prim_set<kSets>(p, n) * p.K + kk) * ((size_t)p.WD * p.WH * p.WW * 3), rec.x, rec.y, rec.z, p);
             else sres = sample_slab<T, V>(tpn + (size_t)kk * slabsz, rec.x, rec.y, rec.z, p.TD, p.TH, p.TW, p.fadescale, p.fadeexp);
         }
         __syncwarp();
@@ -1859,7 +1909,8 @@ __device__ __forceinline__ void clear_grad_slices(const Params &p, size_t g, int
     }
 }
 
-template <int T, bool kGrad, int CAP, bool kWarp, typename V>
+// kSets: a sets call (mvp_raymarch_forward_sets), the primitive set of a view from its map entry (prim_set)
+template <int T, bool kGrad, int CAP, bool kWarp, typename V, bool kSets = false>
 __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_FWD_MINB * 4) / kWarps : 16 / kWarps) render_forward_kernel(const Params p) {
     __shared__ FwdWarpSmem<CAP, kGrad> s_w[kWarps];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -1870,7 +1921,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         for (int i = blockIdx.x * kWarps + warp; i < cnt; i += gridDim.x * kWarps) {
             const int id = p.heavylist[i];
             const int tx = id % p.TXn, ty = (id / p.TXn) % p.TYn, n = id / (p.TXn * p.TYn);
-            forward_tile<T, kGrad, CAP, kWarp, V>(p, n, tx, ty, lane, S);
+            forward_tile<T, kGrad, CAP, kWarp, V, kSets>(p, n, tx, ty, lane, S);
             __syncwarp();
         }
     } else {
@@ -1889,7 +1940,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         long long g0_;
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g0_));
 #endif
-        if (!forward_tile<T, kGrad, CAP, kWarp, V>(p, n, tx, ty, lane, S) && lane == 0)
+        if (!forward_tile<T, kGrad, CAP, kWarp, V, kSets>(p, n, tx, ty, lane, S) && lane == 0)
             p.heavylist[atomicAdd(p.heavycnt, 1)] = (n * p.TYn + ty) * p.TXn + tx;
 #if MVP_TILE_CLOCKS
         if (lane == 0) {
@@ -2031,7 +2082,7 @@ constexpr int kGradAll = 0;         // transforms, template (+ warp field)
 constexpr int kGradNoPayload = 1;   // transforms only (MVP_FLAG_NO_TPLATE_GRAD): no payload-gradient scatter
 constexpr int kGradRaysOnly = 2;    // ray gradients only (MVP_FLAG_RAY_GRADS_ONLY; kRayGrad kernels): no transform sums either
 
-template <int T, int CAP, bool kWarp, typename V, bool kRayGrad, int kSet>
+template <int T, int CAP, bool kWarp, typename V, bool kRayGrad, int kSet, bool kSets>
 __device__ __forceinline__ bool backward_tile(const Params &p, const int n, const int tx, const int ty, const int lane, BwdWarpSmem<CAP> *const S) {
     static_assert(kSet != kGradRaysOnly || kRayGrad, "a rays-only backward computes the ray gradients");
     int *const sk = S->k, *const siv = S->iv;
@@ -2051,7 +2102,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
     have = load_saved_tile_list<CAP>(p, rdt, n, tx, ty, lane, c, sk, siv, xb, yb, zb, j0);
     if (have == 2) return false;
 #endif
-    if (have == 0 && !build_tile_list<CAP, false>(p, rdt, n, tx, ty, lane, c, sk, siv, sstage, sbar, t0, xb, yb, zb, r1e, j0)) return false;
+    if (have == 0 && !build_tile_list<CAP, false, kSets>(p, rdt, n, tx, ty, lane, c, sk, siv, sstage, sbar, t0, xb, yb, zb, r1e, j0)) return false;
     const int nl = c.nl;
     if (nl == 0) {
         if (kRayGrad) store_ray_grads(p, n, tx, ty, lane, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f);
@@ -2100,11 +2151,11 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
         return true;
     }
 
-    const float4 *packn = p.pack + (size_t)(n * p.pview) * p.K * 4;
+    const float4 *packn = p.pack + (size_t)prim_set<kSets>(p, n) * p.K * 4;
     const size_t slabsz = (size_t)p.TD * p.TH * p.TW;   // (a compile-time T^3 here makes the compiler keep slab addresses in registers: 64 B of spills)
     // bases of the primitive tensors are re-derived from the parameter block where they are used (cheap constant-bank
     // arithmetic) instead of living in a dozen registers for the whole tile
-    const size_t pvK = (size_t)(n * p.pview) * p.K;
+    const size_t pvK = (size_t)prim_set<kSets>(p, n) * p.K;
     const int td = T > 0 ? T : p.TD, th = T > 0 ? T : p.TH, tw = T > 0 ? T : p.TW;
     const float gmx = (float)(tw - 1) * 0.5f, gmy = (float)(th - 1) * 0.5f, gmz = (float)(td - 1) * 0.5f;
     const int sx = tw > 1 ? 1 : 0, sy = th > 1 ? tw : 0, sz = td > 1 ? th * tw : 0;
@@ -2173,7 +2224,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                 word &= word - 1;
                 const int slot = w * 32 + bit;
                 const int k = sk[slot];
-                const int rank = rank_of_slab(p.rankof ? p.rankof + (size_t)(n * p.pview) * p.K : nullptr, p.K, kstart, k);
+                const int rank = rank_of_slab(p.rankof ? p.rankof + (size_t)prim_set<kSets>(p, n) * p.K : nullptr, p.K, kstart, k);
 #if MVP_BWD_SMEMREC
                 __syncwarp();                                  // the previous slab's last readers of the record are done
                 if (lane < 4) S->rec[lane] = __ldg(packn + (size_t)k * 4 + lane);
@@ -2461,8 +2512,8 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         } else {
                         // ---- algo 1 (PrimSamplerTW<true>): payload sampled at the warp-field-displaced position ----
                         const size_t wsl = (size_t)p.WD * p.WH * p.WW * 3;
-                        const float *wk = p.warp + ((size_t)(n * p.pview) * p.K + k) * wsl;
-                        float *gwk = kSet == kGradAll ? p.g_warp + ((size_t)(n * p.pview) * p.K + k) * wsl : nullptr;
+                        const float *wk = p.warp + ((size_t)prim_set<kSets>(p, n) * p.K + k) * wsl;
+                        float *gwk = kSet == kGradAll ? p.g_warp + ((size_t)prim_set<kSets>(p, n) * p.K + k) * wsl : nullptr;
                         const float e1 = p.fadeexp - 1.f;
                         const float pw0 = __powf(fabsf(y0), e1), pw1 = __powf(fabsf(y1), e1), pw2 = __powf(fabsf(y2), e1);
                         const float fade = __expf(-p.fadescale * (pw0 * fabsf(y0) + pw1 * fabsf(y1) + pw2 * fabsf(y2)));
@@ -2640,8 +2691,9 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
 }
 
 // kRayGrad: also write the per-ray gradients p.g_raypos / g_raydir / g_tminmax (mvp_raymarch_backward_rays); false compiles to
-// the plain backward.  kSet: the gradient set (kGradAll, kGradNoPayload, kGradRaysOnly); the default is the full backward.
-template <int T, int CAP, bool kWarp, typename V, bool kRayGrad = false, int kSet = kGradAll>
+// the plain backward.  kSet: the gradient set (kGradAll, kGradNoPayload, kGradRaysOnly); the default is the full backward.  kSets: a
+// sets call (mvp_raymarch_backward_sets), as in render_forward_kernel.
+template <int T, int CAP, bool kWarp, typename V, bool kRayGrad = false, int kSet = kGradAll, bool kSets = false>
 __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_BWD_MINB * 4) / kWarps : 12 / kWarps) render_backward_kernel(const Params p) {
     __shared__ typename BwdSmemOf<CAP, kRayGrad>::type s_w[kWarps];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -2651,7 +2703,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         for (int i = blockIdx.x * kWarps + warp; i < cnt; i += gridDim.x * kWarps) {
             const int id = p.heavylist[i];
             const int tx = id % p.TXn, ty = (id / p.TXn) % p.TYn, n = id / (p.TXn * p.TYn);
-            backward_tile<T, CAP, kWarp, V, kRayGrad, kSet>(p, n, tx, ty, lane, S);
+            backward_tile<T, CAP, kWarp, V, kRayGrad, kSet, kSets>(p, n, tx, ty, lane, S);
             __syncwarp();
         }
     } else {
@@ -2664,7 +2716,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         const int tx = blockIdx.x * kBlkTX + (warp % kBlkTX), ty = blockIdx.y * kBlkTY + (warp / kBlkTX), n = blockIdx.z;
 #endif
         if (tx >= p.TXn || ty >= p.TYn) return;
-        if (!backward_tile<T, CAP, kWarp, V, kRayGrad, kSet>(p, n, tx, ty, lane, S) && lane == 0)
+        if (!backward_tile<T, CAP, kWarp, V, kRayGrad, kSet, kSets>(p, n, tx, ty, lane, S) && lane == 0)
             p.heavylist[atomicAdd(p.heavycnt, 1)] = (n * p.TYn + ty) * p.TXn + tx;
     }
 }
@@ -2720,9 +2772,11 @@ int check_shape(const mvp_shape &s) {
     return MVP_OK;
 }
 
-// camera: NULL or a checked mvp_camera (then raypos / raydir are not used)
-int launch_accel(const mvp_shape &s, int pview, const int *order, const float *raypos, const float *raydir, const mvp_camera *camera,
-                 const float *primpos, const float *primrot, const float *primscale, char *ws, const Layout &L, cudaStream_t st) {
+// camera: NULL or a checked mvp_camera (then raypos / raydir are not used); vset: NULL, or the view -> set map of a sets call
+// (then pview is ignored, and the primitive tensors and order hold nsets sets)
+int launch_accel(const mvp_shape &s, int pview, const int *vset, int nsets, const int *order, const float *raypos, const float *raydir,
+                 const mvp_camera *camera, const float *primpos, const float *primrot, const float *primscale, char *ws, const Layout &L,
+                 cudaStream_t st) {
     const int ostride = pview ? s.K : 0;      // the order belongs to the primitives: one per view, or one shared by all views
     Cam *cam = reinterpret_cast<Cam *>(ws + L.cam);
     int *bad = reinterpret_cast<int *>(ws + L.bad);
@@ -2745,19 +2799,19 @@ int launch_accel(const mvp_shape &s, int pview, const int *order, const float *r
     else
         MVP_LAUNCH(fit_camera_kernel, gfit, kFitThreads, 0, st, s.H, s.W, raypos, raydir, cam, bad);
     const size_t NK = (size_t)s.N * s.K;
-    MVP_LAUNCH(prim_setup_kernel, (unsigned)((NK + 127) / 128), 128, 0, st, s.N, s.K, s.H, s.W, pview, primpos, primrot, primscale, cam, bad,
+    MVP_LAUNCH(prim_setup_kernel, (unsigned)((NK + 127) / 128), 128, 0, st, s.N, s.K, s.H, s.W, pview, vset, nsets, primpos, primrot, primscale, cam, bad,
                reinterpret_cast<float4 *>(ws + L.pack), reinterpret_cast<unsigned *>(ws + L.rx), reinterpret_cast<unsigned *>(ws + L.ry));
     const int TXn = (s.W + kTileW - 1) / kTileW;
     if (order) {
-        const size_t nk = (size_t)(pview ? s.N : 1) * s.K;
+        const size_t nk = (size_t)(vset ? nsets : pview ? s.N : 1) * s.K;
         MVP_LAUNCH(invert_order_kernel, (unsigned)((nk + 255) / 256), 256, 0, st, nk, s.K, order, reinterpret_cast<int *>(ws + L.rankof));
     }
     MVP_LAUNCH(block_ranges_kernel, dim3(((s.K + 31) / 32 + 7) / 8, s.N), 256, 0, st, s.K, reinterpret_cast<const unsigned *>(ws + L.ry),
-               order, ostride, reinterpret_cast<unsigned *>(ws + L.blky));
+               order, ostride, vset, nsets, reinterpret_cast<unsigned *>(ws + L.blky));
     if (small_launch)
         MVP_LAUNCH(row_lists_cta_kernel, dim3(L.R, s.N), kRowThreads, 0, st, s.K, L.R, L.rowcap, TXn,
                    reinterpret_cast<unsigned *>(ws + L.rx), reinterpret_cast<unsigned *>(ws + L.ry),
-                   reinterpret_cast<const unsigned *>(ws + L.blky), order, ostride, reinterpret_cast<int *>(ws + L.rowcnt),
+                   reinterpret_cast<const unsigned *>(ws + L.blky), order, ostride, vset, nsets, reinterpret_cast<int *>(ws + L.rowcnt),
                    reinterpret_cast<RowEntry *>(ws + L.rowlist)
 #if MVP_XBUCKETS
                    , L.NG, reinterpret_cast<int2 *>(ws + L.grphdr), reinterpret_cast<RowEntry *>(ws + L.grplist),
@@ -2767,7 +2821,7 @@ int launch_accel(const mvp_shape &s, int pview, const int *order, const float *r
     else
         MVP_LAUNCH(row_lists_kernel, dim3((L.R + kRowThreads / 32 - 1) / (kRowThreads / 32), s.N), kRowThreads, 0, st, s.K, L.R, L.rowcap, TXn,
                    reinterpret_cast<unsigned *>(ws + L.rx), reinterpret_cast<unsigned *>(ws + L.ry),
-                   reinterpret_cast<const unsigned *>(ws + L.blky), order, ostride, reinterpret_cast<int *>(ws + L.rowcnt),
+                   reinterpret_cast<const unsigned *>(ws + L.blky), order, ostride, vset, nsets, reinterpret_cast<int *>(ws + L.rowcnt),
                    reinterpret_cast<RowEntry *>(ws + L.rowlist)
 #if MVP_XBUCKETS
                    , L.NG, reinterpret_cast<int2 *>(ws + L.grphdr), reinterpret_cast<RowEntry *>(ws + L.grplist),
@@ -2782,19 +2836,19 @@ int launch_accel(const mvp_shape &s, int pview, const int *order, const float *r
         fit_camera_kernel<<<gfit, kFitThreads, 0, st>>>(s.H, s.W, raypos, raydir, cam, bad);
     const size_t NK = (size_t)s.N * s.K;
     prim_setup_kernel<<<(unsigned)((NK + 127) / 128), 128, 0, st>>>(
-        s.N, s.K, s.H, s.W, pview, primpos, primrot, primscale, cam, bad, reinterpret_cast<float4 *>(ws + L.pack),
+        s.N, s.K, s.H, s.W, pview, vset, nsets, primpos, primrot, primscale, cam, bad, reinterpret_cast<float4 *>(ws + L.pack),
         reinterpret_cast<unsigned *>(ws + L.rx), reinterpret_cast<unsigned *>(ws + L.ry));
     const int TXn = (s.W + kTileW - 1) / kTileW;
     if (order) {
-        const size_t nk = (size_t)(pview ? s.N : 1) * s.K;
+        const size_t nk = (size_t)(vset ? nsets : pview ? s.N : 1) * s.K;
         invert_order_kernel<<<(unsigned)((nk + 255) / 256), 256, 0, st>>>(nk, s.K, order, reinterpret_cast<int *>(ws + L.rankof));
     }
     block_ranges_kernel<<<dim3(((s.K + 31) / 32 + 7) / 8, s.N), 256, 0, st>>>(s.K, reinterpret_cast<const unsigned *>(ws + L.ry), order,
-                                                                               ostride, reinterpret_cast<unsigned *>(ws + L.blky));
+                                                                               ostride, vset, nsets, reinterpret_cast<unsigned *>(ws + L.blky));
     if (small_launch)
         row_lists_cta_kernel<<<dim3(L.R, s.N), kRowThreads, 0, st>>>(
             s.K, L.R, L.rowcap, TXn, reinterpret_cast<unsigned *>(ws + L.rx), reinterpret_cast<unsigned *>(ws + L.ry),
-            reinterpret_cast<const unsigned *>(ws + L.blky), order, ostride, reinterpret_cast<int *>(ws + L.rowcnt),
+            reinterpret_cast<const unsigned *>(ws + L.blky), order, ostride, vset, nsets, reinterpret_cast<int *>(ws + L.rowcnt),
             reinterpret_cast<RowEntry *>(ws + L.rowlist)
 #if MVP_XBUCKETS
             , L.NG, reinterpret_cast<int2 *>(ws + L.grphdr), reinterpret_cast<RowEntry *>(ws + L.grplist),
@@ -2804,7 +2858,7 @@ int launch_accel(const mvp_shape &s, int pview, const int *order, const float *r
     else
         row_lists_kernel<<<dim3((L.R + kRowThreads / 32 - 1) / (kRowThreads / 32), s.N), kRowThreads, 0, st>>>(
             s.K, L.R, L.rowcap, TXn, reinterpret_cast<unsigned *>(ws + L.rx), reinterpret_cast<unsigned *>(ws + L.ry),
-            reinterpret_cast<const unsigned *>(ws + L.blky), order, ostride, reinterpret_cast<int *>(ws + L.rowcnt),
+            reinterpret_cast<const unsigned *>(ws + L.blky), order, ostride, vset, nsets, reinterpret_cast<int *>(ws + L.rowcnt),
             reinterpret_cast<RowEntry *>(ws + L.rowlist)
 #if MVP_XBUCKETS
             , L.NG, reinterpret_cast<int2 *>(ws + L.grphdr), reinterpret_cast<RowEntry *>(ws + L.grplist),
@@ -2886,7 +2940,7 @@ const char *mvp_build_config(void) {
     return "LIST_REUSE=" MVP_STR(MVP_LIST_REUSE)
            " LIST_MARGIN=" MVP_STR(MVP_LIST_MARGIN) " XBUCKETS=" MVP_STR(MVP_XBUCKETS) " FASTCAP=" MVP_STR(MVP_FWD_FASTCAP) "/" MVP_STR(MVP_BWD_FASTCAP) " SMEM_UNION=" MVP_STR(MVP_SMEM_UNION) " CARVEOUT=" MVP_STR(MVP_FWD_CARVEOUT) "/" MVP_STR(MVP_BWD_CARVEOUT) " FWD_RING=" MVP_STR(MVP_FWD_RING) " BWD_SMEMREC=" MVP_STR(MVP_BWD_SMEMREC) " BWD_LANESMEM=" MVP_STR(MVP_BWD_LANESMEM) " CTA_ORDER=" MVP_STR(MVP_CTA_ORDER) " CTA_ORDER_MIN=" MVP_STR(MVP_CTA_ORDER_MIN)
            " CHUNK=" MVP_STR(MVP_CHUNK) " FWD_MINB=" MVP_STR(MVP_FWD_MINB) " BWD_MINB=" MVP_STR(MVP_BWD_MINB)
-           " WARPS=" MVP_STR(MVP_WARPS) " BLK_TX=" MVP_STR(MVP_BLK_TX) " TPLATE_BF16=1 EPILOGUE_BF16=1 RAY_GRADS=1 GRAD_TPLATE_F32=1 GRAD_SELECT=1"
+           " WARPS=" MVP_STR(MVP_WARPS) " BLK_TX=" MVP_STR(MVP_BLK_TX) " TPLATE_BF16=1 EPILOGUE_BF16=1 RAY_GRADS=1 GRAD_TPLATE_F32=1 GRAD_SELECT=1 VIEW_SETS=1"
 #ifdef MVP_CPU_EMUL
            " CPU_EMUL"
 #endif
@@ -2921,7 +2975,7 @@ int mvp_build_accel(const mvp_shape *shape, uint32_t flags, const int32_t *order
     if (rc != MVP_OK) return rc;
     const Layout L = make_layout(*shape);
     if (workspace_bytes < L.total || ((uintptr_t)workspace & 255)) return MVP_ERR_WORKSPACE;
-    return launch_accel(*shape, (flags & MVP_FLAG_SHARED_PRIMS) ? 0 : 1, order, raypos, raydir, nullptr, primpos, primrot, primscale,
+    return launch_accel(*shape, (flags & MVP_FLAG_SHARED_PRIMS) ? 0 : 1, nullptr, 0, order, raypos, raydir, nullptr, primpos, primrot, primscale,
                         (char *)workspace, L, (cudaStream_t)stream);
 }
 
@@ -2944,7 +2998,7 @@ int mvp_build_accel_camera(const mvp_shape *shape, uint32_t flags, const int32_t
     if (rc <= 0) return rc == 0 ? MVP_ERR_NULL : rc;
     const Layout L = make_layout(*shape);
     if (workspace_bytes < L.total || ((uintptr_t)workspace & 255)) return MVP_ERR_WORKSPACE;
-    return launch_accel(*shape, (flags & MVP_FLAG_SHARED_PRIMS) ? 0 : 1, order, nullptr, nullptr, camera, primpos, primrot, primscale,
+    return launch_accel(*shape, (flags & MVP_FLAG_SHARED_PRIMS) ? 0 : 1, nullptr, 0, order, nullptr, nullptr, camera, primpos, primrot, primscale,
                         (char *)workspace, L, (cudaStream_t)stream);
 }
 
@@ -2988,9 +3042,15 @@ static inline unsigned grad_tplate_words(uint32_t flags) {
     return ((flags & MVP_FLAG_TPLATE_BF16) && !(flags & MVP_FLAG_GRAD_TPLATE_F32)) ? Payload<Bf16x4>::kWords : Payload<float4>::kWords;
 }
 
-int mvp_raymarch_forward(const mvp_forward_args *a, void *stream) {
-    if (!a) return MVP_ERR_NULL;
-    if (a->struct_size != sizeof(mvp_forward_args)) return MVP_ERR_STRUCT;
+// The argument errors of a sets call (mvp_raymarch_forward_sets / mvp_raymarch_backward_sets), given a checked struct
+static int check_view_sets(const mvp_shape &s, uint32_t flags, const int32_t *view_set, int32_t nsets) {
+    if (!view_set) return MVP_ERR_NULL;
+    if (nsets < 1 || nsets > s.N || (flags & MVP_FLAG_SHARED_PRIMS)) return MVP_ERR_SHAPE;
+    return misaligned(view_set, 4) ? MVP_ERR_ALIGN : MVP_OK;
+}
+
+// mvp_raymarch_forward, and with vset != NULL mvp_raymarch_forward_sets (struct and map checked by the caller)
+static int forward_impl(const mvp_forward_args *a, const int32_t *vset, int nsets, void *stream) {
     const int camrc = check_camera(a->camera);
     if (camrc < 0) return camrc;
     const mvp_camera *const camera = camrc ? &a->camera : nullptr;      // rays generated in the kernels: the ray tensors are not read
@@ -3025,12 +3085,14 @@ int mvp_raymarch_forward(const mvp_forward_args *a, void *stream) {
     char *ws = (char *)a->workspace;
     const int pview = (a->flags & MVP_FLAG_SHARED_PRIMS) ? 0 : 1;
     if (!(a->flags & MVP_FLAG_ACCEL_VALID)) {
-        rc = launch_accel(a->shape, pview, a->order, a->raypos, a->raydir, camera, a->primpos, a->primrot, a->primscale, ws, L, st);
+        rc = launch_accel(a->shape, pview, vset, nsets, a->order, a->raypos, a->raydir, camera, a->primpos, a->primrot, a->primscale, ws,
+                          L, st);
         if (rc != MVP_OK) return rc;
     }
     Params p{};
     fill_params(p, a->shape, a->stepsize, a->fadescale, a->fadeexp, ws, L, bf16 ? Payload<Bf16x4>::kBytes : Payload<float4>::kBytes);
     p.pview = pview;
+    p.vset = vset; p.nsets = nsets;
     p.raycam = camera ? reinterpret_cast<const float4 *>(ws + L.raycam) : nullptr;
     p.order = a->order; p.rankof = a->order ? reinterpret_cast<const int *>(ws + L.rankof) : nullptr;
     p.rgb_nchw = a->rayrgb_nchw; p.alpha_nchw = a->rayalpha_nchw;
@@ -3053,7 +3115,7 @@ int mvp_raymarch_forward(const mvp_forward_args *a, void *stream) {
     }
     if (a->raysat) {
         // gradient buffers to clear for the coming backward: in the fast render kernel (one slice per warp), see clear_grad_slices
-        const size_t nk = (size_t)(pview ? a->shape.N : 1) * a->shape.K;
+        const size_t nk = (size_t)(vset ? nsets : pview ? a->shape.N : 1) * a->shape.K;
         float *const bufs[kClearBufs] = {clr_primpos, clr_primrot, clr_primscale, clr_tplate, a->algo == 1 ? clr_warp : nullptr};
         // sizes in 4-byte words: a bf16 template gradient holds two channels per word
         const size_t floats[kClearBufs] = {nk * 3, nk * 9, nk * 3, nk * a->shape.TD * a->shape.TH * a->shape.TW * grad_tplate_words(a->flags),
@@ -3078,36 +3140,55 @@ int mvp_raymarch_forward(const mvp_forward_args *a, void *stream) {
     const int cubic = (a->shape.TD == a->shape.TH && a->shape.TH == a->shape.TW) ? a->shape.TD : 0;
     int heavy = 0;
     if (int eh = heavy_grid(&heavy)) return eh;
-#define MVP_LAUNCH_FWD(TT, WW_, VV)                                                                          \
+#define MVP_LAUNCH_FWD(TT, WW_, VV, SS)                                                                      \
     do {                                                                                                     \
         if (a->raysat) {                                                                                     \
-            MVP_CARVE(MVP_FWD_CARVEOUT, render_forward_kernel<TT, true, kFastCapF, WW_, VV>);                \
-            MVP_LAUNCH_FAST(render_forward_kernel<TT, true, kFastCapF, WW_, VV>);                            \
-            MVP_LAUNCH_HEAVY(render_forward_kernel<TT, true, kMaxHit, WW_, VV>);                             \
+            MVP_CARVE(MVP_FWD_CARVEOUT, render_forward_kernel<TT, true, kFastCapF, WW_, VV, SS>);            \
+            MVP_LAUNCH_FAST(render_forward_kernel<TT, true, kFastCapF, WW_, VV, SS>);                        \
+            MVP_LAUNCH_HEAVY(render_forward_kernel<TT, true, kMaxHit, WW_, VV, SS>);                         \
         } else {                                                                                             \
-            MVP_CARVE(MVP_FWD_CARVEOUT, render_forward_kernel<TT, false, kFastCapF, WW_, VV>);               \
-            MVP_LAUNCH_FAST(render_forward_kernel<TT, false, kFastCapF, WW_, VV>);                           \
-            MVP_LAUNCH_HEAVY(render_forward_kernel<TT, false, kMaxHit, WW_, VV>);                            \
+            MVP_CARVE(MVP_FWD_CARVEOUT, render_forward_kernel<TT, false, kFastCapF, WW_, VV, SS>);           \
+            MVP_LAUNCH_FAST(render_forward_kernel<TT, false, kFastCapF, WW_, VV, SS>);                       \
+            MVP_LAUNCH_HEAVY(render_forward_kernel<TT, false, kMaxHit, WW_, VV, SS>);                        \
         }                                                                                                    \
     } while (0)
-#define MVP_LAUNCH_FWD_T(VV)                                                                                 \
+#define MVP_LAUNCH_FWD_T(VV, SS)                                                                             \
     do {                                                                                                     \
-        if (a->algo == 1) MVP_LAUNCH_FWD(0, true, VV);                                                       \
-        else if (cubic == 8) MVP_LAUNCH_FWD(8, false, VV);                                                   \
-        else if (cubic == 16) MVP_LAUNCH_FWD(16, false, VV);                                                 \
-        else MVP_LAUNCH_FWD(0, false, VV);                                                                   \
+        if (a->algo == 1) MVP_LAUNCH_FWD(0, true, VV, SS);                                                   \
+        else if (cubic == 8) MVP_LAUNCH_FWD(8, false, VV, SS);                                               \
+        else if (cubic == 16) MVP_LAUNCH_FWD(16, false, VV, SS);                                             \
+        else MVP_LAUNCH_FWD(0, false, VV, SS);                                                               \
     } while (0)
-    if (bf16) MVP_LAUNCH_FWD_T(Bf16x4);
-    else MVP_LAUNCH_FWD_T(float4);
+    if (vset) {
+        if (bf16) MVP_LAUNCH_FWD_T(Bf16x4, true);
+        else MVP_LAUNCH_FWD_T(float4, true);
+    } else {
+        if (bf16) MVP_LAUNCH_FWD_T(Bf16x4, false);
+        else MVP_LAUNCH_FWD_T(float4, false);
+    }
 #undef MVP_LAUNCH_FWD_T
 #undef MVP_LAUNCH_FWD
     cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? MVP_OK : (int)e;
 }
 
+int mvp_raymarch_forward(const mvp_forward_args *a, void *stream) {
+    if (!a) return MVP_ERR_NULL;
+    if (a->struct_size != sizeof(mvp_forward_args)) return MVP_ERR_STRUCT;
+    return forward_impl(a, nullptr, 0, stream);
+}
+
+int mvp_raymarch_forward_sets(const mvp_forward_args *a, const int32_t *view_set, int32_t nsets, void *stream) {
+    if (!a) return MVP_ERR_NULL;
+    if (a->struct_size != sizeof(mvp_forward_args)) return MVP_ERR_STRUCT;
+    const int rc = check_view_sets(a->shape, a->flags, view_set, nsets);
+    return rc != MVP_OK ? rc : forward_impl(a, view_set, nsets, stream);
+}
+
 // mvp_raymarch_backward, and with rays = true mvp_raymarch_backward_rays (grad_raypos / grad_raydir / grad_tminmax checked by the caller
-// for NULL; every other check is made here, before any device work)
-static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_raypos, float *grad_raydir, float *grad_tminmax, void *stream) {
+// for NULL; every other check is made here, before any device work); vset != NULL: the sets forms (map checked by the caller)
+static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_raypos, float *grad_raydir, float *grad_tminmax,
+                         const int32_t *vset, int nsets, void *stream) {
     const int camrc = check_camera(a->camera);
     if (camrc < 0) return camrc;
     const mvp_camera *const camera = camrc ? &a->camera : nullptr;
@@ -3146,11 +3227,12 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
     char *ws = (char *)a->workspace;
     const int pview = (a->flags & MVP_FLAG_SHARED_PRIMS) ? 0 : 1;
     if (!(a->flags & MVP_FLAG_ACCEL_VALID)) {
-        rc = launch_accel(a->shape, pview, a->order, a->raypos, a->raydir, camera, a->primpos, a->primrot, a->primscale, ws, L, st);
+        rc = launch_accel(a->shape, pview, vset, nsets, a->order, a->raypos, a->raydir, camera, a->primpos, a->primrot, a->primscale, ws,
+                          L, st);
         if (rc != MVP_OK) return rc;
     }
     if (a->flags & MVP_FLAG_ZERO_GRADS) {     // the requested buffers only
-        const size_t nk = (size_t)(pview ? a->shape.N : 1) * a->shape.K;
+        const size_t nk = (size_t)(vset ? nsets : pview ? a->shape.N : 1) * a->shape.K;
         cudaError_t z = cudaSuccess;
         if (gp) z = cudaMemsetAsync(grad_primpos, 0, nk * 3 * sizeof(float), st);
         if (gp && z == cudaSuccess) z = cudaMemsetAsync(grad_primrot, 0, nk * 9 * sizeof(float), st);
@@ -3163,6 +3245,7 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
     Params p{};
     fill_params(p, a->shape, a->stepsize, a->fadescale, a->fadeexp, ws, L, bf16 ? Payload<Bf16x4>::kBytes : Payload<float4>::kBytes);
     p.pview = pview;
+    p.vset = vset; p.nsets = nsets;
     p.raycam = camera ? reinterpret_cast<const float4 *>(ws + L.raycam) : nullptr;
     p.raypos = a->raypos; p.raydir = a->raydir; p.tminmax = a->tminmax; p.tplate = a->tplate;
     p.use_order = a->shape.N <= MVP_CTA_ORDER_MAXVIEWS;
@@ -3185,42 +3268,48 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
     const int cubic = (a->shape.TD == a->shape.TH && a->shape.TH == a->shape.TW) ? a->shape.TD : 0;
     int heavy = 0;
     if (int eh = heavy_grid(&heavy)) return eh;
-#define MVP_LAUNCH_BWD(TT, WW_, VV)                                                                          \
+#define MVP_LAUNCH_BWD(TT, WW_, VV, SS)                                                                      \
     do {                                                                                                     \
         if (rays) {                                                                                          \
-            MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV, true>);               \
-            MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV, true>);                           \
-            MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV, true>);                            \
+            MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV, true, kGradAll, SS>); \
+            MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV, true, kGradAll, SS>);             \
+            MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV, true, kGradAll, SS>);              \
         } else {                                                                                             \
-            MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV>);                     \
-            MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV>);                                 \
-            MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV>);                                  \
+            MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV, false, kGradAll, SS>);\
+            MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV, false, kGradAll, SS>);            \
+            MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV, false, kGradAll, SS>);             \
         }                                                                                                    \
     } while (0)
     // the reduced gradient sets (float4 and Bf16x4 only: without a template gradient Bf16x4G32 is Bf16x4)
-#define MVP_LAUNCH_BWD_SET(TT, WW_, VV, RG, SET)                                                             \
+#define MVP_LAUNCH_BWD_SET(TT, WW_, VV, RG, SET, SS)                                                         \
     do {                                                                                                     \
-        MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV, RG, SET>);                \
-        MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV, RG, SET>);                            \
-        MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV, RG, SET>);                             \
+        MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV, RG, SET, SS>);            \
+        MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV, RG, SET, SS>);                        \
+        MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV, RG, SET, SS>);                         \
     } while (0)
-#define MVP_LAUNCH_BWD_ANY(TT, WW_, VV)                                                                      \
+#define MVP_LAUNCH_BWD_ANY(TT, WW_, VV, SS)                                                                  \
     do {                                                                                                     \
-        if (set == kGradRaysOnly) MVP_LAUNCH_BWD_SET(TT, WW_, VV, true, kGradRaysOnly);                      \
-        else if (set == kGradNoPayload && rays) MVP_LAUNCH_BWD_SET(TT, WW_, VV, true, kGradNoPayload);       \
-        else if (set == kGradNoPayload) MVP_LAUNCH_BWD_SET(TT, WW_, VV, false, kGradNoPayload);              \
-        else MVP_LAUNCH_BWD(TT, WW_, VV);                                                                    \
+        if (set == kGradRaysOnly) MVP_LAUNCH_BWD_SET(TT, WW_, VV, true, kGradRaysOnly, SS);                  \
+        else if (set == kGradNoPayload && rays) MVP_LAUNCH_BWD_SET(TT, WW_, VV, true, kGradNoPayload, SS);   \
+        else if (set == kGradNoPayload) MVP_LAUNCH_BWD_SET(TT, WW_, VV, false, kGradNoPayload, SS);          \
+        else MVP_LAUNCH_BWD(TT, WW_, VV, SS);                                                                \
     } while (0)
-#define MVP_LAUNCH_BWD_T(LAUNCH, VV)                                                             \
+#define MVP_LAUNCH_BWD_T(LAUNCH, VV, SS)                                                         \
     do {                                                                                         \
-        if (a->algo == 1) LAUNCH(0, true, VV);                                                   \
-        else if (cubic == 8) LAUNCH(8, false, VV);                                               \
-        else if (cubic == 16) LAUNCH(16, false, VV);                                             \
-        else LAUNCH(0, false, VV);                                                               \
+        if (a->algo == 1) LAUNCH(0, true, VV, SS);                                               \
+        else if (cubic == 8) LAUNCH(8, false, VV, SS);                                           \
+        else if (cubic == 16) LAUNCH(16, false, VV, SS);                                         \
+        else LAUNCH(0, false, VV, SS);                                                           \
     } while (0)
-    if (bf16 && gwords == Payload<Bf16x4G32>::kWords && set == kGradAll) MVP_LAUNCH_BWD_T(MVP_LAUNCH_BWD, Bf16x4G32);
-    else if (bf16) MVP_LAUNCH_BWD_T(MVP_LAUNCH_BWD_ANY, Bf16x4);
-    else MVP_LAUNCH_BWD_T(MVP_LAUNCH_BWD_ANY, float4);
+#define MVP_LAUNCH_BWD_V(SS)                                                                                 \
+    do {                                                                                                     \
+        if (bf16 && gwords == Payload<Bf16x4G32>::kWords && set == kGradAll) MVP_LAUNCH_BWD_T(MVP_LAUNCH_BWD, Bf16x4G32, SS); \
+        else if (bf16) MVP_LAUNCH_BWD_T(MVP_LAUNCH_BWD_ANY, Bf16x4, SS);                                     \
+        else MVP_LAUNCH_BWD_T(MVP_LAUNCH_BWD_ANY, float4, SS);                                               \
+    } while (0)
+    if (vset) MVP_LAUNCH_BWD_V(true);
+    else MVP_LAUNCH_BWD_V(false);
+#undef MVP_LAUNCH_BWD_V
 #undef MVP_LAUNCH_BWD_T
 #undef MVP_LAUNCH_BWD_ANY
 #undef MVP_LAUNCH_BWD_SET
@@ -3232,14 +3321,24 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
 int mvp_raymarch_backward(const mvp_backward_args *a, void *stream) {
     if (!a) return MVP_ERR_NULL;
     if (a->struct_size != sizeof(mvp_backward_args)) return MVP_ERR_STRUCT;
-    return backward_impl(a, false, nullptr, nullptr, nullptr, stream);
+    return backward_impl(a, false, nullptr, nullptr, nullptr, nullptr, 0, stream);
 }
 
 int mvp_raymarch_backward_rays(const mvp_backward_args *a, float *grad_raypos, float *grad_raydir, float *grad_tminmax, void *stream) {
     if (!a) return MVP_ERR_NULL;
     if (a->struct_size != sizeof(mvp_backward_args)) return MVP_ERR_STRUCT;
     if (!grad_raypos || !grad_raydir || !grad_tminmax) return MVP_ERR_NULL;
-    return backward_impl(a, true, grad_raypos, grad_raydir, grad_tminmax, stream);
+    return backward_impl(a, true, grad_raypos, grad_raydir, grad_tminmax, nullptr, 0, stream);
+}
+
+int mvp_raymarch_backward_sets(const mvp_backward_args *a, const int32_t *view_set, int32_t nsets, float *grad_raypos, float *grad_raydir,
+                               float *grad_tminmax, void *stream) {
+    if (!a) return MVP_ERR_NULL;
+    if (a->struct_size != sizeof(mvp_backward_args)) return MVP_ERR_STRUCT;
+    const int nrays = (grad_raypos != nullptr) + (grad_raydir != nullptr) + (grad_tminmax != nullptr);
+    if (nrays != 0 && nrays != 3) return MVP_ERR_NULL;
+    const int rc = check_view_sets(a->shape, a->flags, view_set, nsets);
+    return rc != MVP_OK ? rc : backward_impl(a, nrays == 3, grad_raypos, grad_raydir, grad_tminmax, view_set, nsets, stream);
 }
 
 #if defined(MVP_CPU_EMUL) && defined(MVP_EMUL_STATS)

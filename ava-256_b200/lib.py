@@ -87,7 +87,8 @@ EXPORTS = ("mvp_abi_version", "mvp_build_config", "mvp_error_string", "mvp_works
            "mvp_assemble_payload_backward", "mvp_debug_saved_tiles", "mvp_debug_tileclk_offset", "mvp_debug_heavy_offset",
            "mvp_compute_morton",
            "mvp_expand_views", "mvp_sum_views", "mvp_assemble_payload_forward_bf16", "mvp_assemble_payload_backward_bf16",
-           "mvp_sum_views_bf16", "mvp_raymarch_backward_rays", "mvp_compute_raydirs_backward")
+           "mvp_sum_views_bf16", "mvp_raymarch_backward_rays", "mvp_compute_raydirs_backward", "mvp_raymarch_forward_sets",
+           "mvp_raymarch_backward_sets")
 
 
 def _load():
@@ -126,6 +127,10 @@ def _load():
     lib.mvp_compute_raydirs.argtypes = [ctypes.c_int32] * 3 + [c_f] * 5 + [ctypes.c_float] + [c_f] * 4
     lib.mvp_raymarch_backward_rays.restype = ctypes.c_int
     lib.mvp_raymarch_backward_rays.argtypes = [ctypes.POINTER(BackwardArgs)] + [c_f] * 4
+    lib.mvp_raymarch_forward_sets.restype = ctypes.c_int
+    lib.mvp_raymarch_forward_sets.argtypes = [ctypes.POINTER(ForwardArgs), c_f, ctypes.c_int32, c_f]
+    lib.mvp_raymarch_backward_sets.restype = ctypes.c_int
+    lib.mvp_raymarch_backward_sets.argtypes = [ctypes.POINTER(BackwardArgs), c_f, ctypes.c_int32] + [c_f] * 4
     lib.mvp_compute_raydirs_backward.restype = ctypes.c_int
     lib.mvp_compute_raydirs_backward.argtypes = [ctypes.c_int32] * 3 + [c_f] * 5 + [ctypes.c_float] + [c_f] * 8
     lib.mvp_composite_forward.restype = ctypes.c_int
@@ -204,6 +209,13 @@ def require_grad_select():
     as GRAD_SELECT=1 in its build configuration.  An older library ignores the two bits and would write to NULL buffers."""
     if "GRAD_SELECT=1" not in LIB.mvp_build_config().decode().split():
         raise RuntimeError("mvpraymarch_b200: this library (%s) does not support reduced gradient sets" % _build.LIB)
+
+
+def require_view_sets():
+    """Raise unless the library renders several primitive sets in one launch (mvp_raymarch_forward_sets,
+    mvp_raymarch_backward_sets), which it reports as VIEW_SETS=1 in its build configuration."""
+    if "VIEW_SETS=1" not in LIB.mvp_build_config().decode().split():
+        raise RuntimeError("mvpraymarch_b200: this library (%s) does not support per-view primitive sets" % _build.LIB)
 
 
 def workspace_bytes(N, H, W, K, TD, TH, TW):

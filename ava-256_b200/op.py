@@ -17,6 +17,7 @@ everything else (mvpraymarch.py:279-292).  Differences that are deliberate:
 """
 import contextlib
 import ctypes
+import numbers
 
 import torch
 from torch.autograd import Function
@@ -204,12 +205,17 @@ class MVPRaymarch(Function):
         if camera is None:
             assert raydir.shape[:3] == (N, H, W) and tminmax.shape[:3] == (N, H, W), "raypos / raydir / tminmax disagree on [N,H,W]"
         NP = primpos.size(0)
-        assert NP in (N, 1), "primitive batch (%d) must equal the number of views (%d) or be 1 (shared)" % (NP, N)
+        view_set = options.get("_view_set")     # per-view primitive sets (mvpraymarch_sets): NP sets, chosen per view by the map
+        if view_set is not None:
+            _lib.require_view_sets()
+            view_set = _view_set_tensor(view_set, N, NP, dev)
+        else:
+            assert NP in (N, 1), "primitive batch (%d) must equal the number of views (%d) or be 1 (shared)" % (NP, N)
         assert primrot.shape[:2] == (NP, K) and primscale.shape[:2] == (NP, K) and template.shape[:2] == (NP, K), \
             "primpos / primrot / primscale / template disagree on [N,K]"
         if warp is not None:
             assert warp.shape[:2] == (NP, K), "warp disagrees with the primitives on [N,K]"
-        shared = NP == 1 and N > 1
+        shared = view_set is None and NP == 1 and N > 1
         template, tminmax = _aligned(template, 8 if bf16 else 16), _aligned(tminmax, 8)
         with torch.cuda.device(dev):
             wsbytes = _lib.workspace_bytes(N, H, W, K, TD, TH, TW)
@@ -256,7 +262,10 @@ class MVPRaymarch(Function):
                 a.clear_grad_primpos, a.clear_grad_primrot, a.clear_grad_primscale = _ptr(grads[0]), _ptr(grads[1]), _ptr(grads[2])
                 a.clear_grad_tplate, a.clear_grad_warp = _ptr(grads[3]), _ptr(grads[4])
             stream = torch.cuda.current_stream(dev).cuda_stream
-            _lib.check(_lib.LIB.mvp_raymarch_forward(ctypes.byref(a), ctypes.c_void_p(stream)))
+            if view_set is not None:
+                _lib.check(_lib.LIB.mvp_raymarch_forward_sets(ctypes.byref(a), _ptr(view_set), NP, ctypes.c_void_p(stream)))
+            else:
+                _lib.check(_lib.LIB.mvp_raymarch_forward(ctypes.byref(a), ctypes.c_void_p(stream)))
 
         if gradmode:
             ctx.grads = grads
@@ -268,6 +277,7 @@ class MVPRaymarch(Function):
             ctx.options = options
             ctx.stepsize = float(stepsize)
             ctx.shared = shared
+            ctx.view_set = view_set
             ctx.tflags = tflags
         if planes:
             return rayrgb, rayalpha
@@ -343,6 +353,10 @@ def _march_backward(ctx, grad_rayrgba, grad_rayalpha, want_rays):
             _lib.require_ray_grads()
             # written for every ray by the library: no zero-fill
             rays = (torch.empty((N, H, W, 3), device=dev), torch.empty((N, H, W, 3), device=dev), torch.empty((N, H, W, 2), device=dev))
+        if ctx.view_set is not None:
+            _lib.check(_lib.LIB.mvp_raymarch_backward_sets(ctypes.byref(a), _ptr(ctx.view_set), primpos.size(0),
+                                                           *(_ptr(t) for t in (rays or (None,) * 3)), stream))
+        elif want_rays:
             _lib.check(_lib.LIB.mvp_raymarch_backward_rays(ctypes.byref(a), *(_ptr(t) for t in rays), stream))
         else:
             _lib.check(_lib.LIB.mvp_raymarch_backward(ctypes.byref(a), stream))
@@ -495,6 +509,8 @@ def mvpraymarch(
         "fadeexp": fadeexp, "accum": accum, "termthresh": termthresh, "griddim": griddim, "blocksize": blocksize,
         "bwdblocksize": bwdblocksize, "_order": order, "_template_grad_dtype": _TEMPLATE_GRAD.get("dtype"),
     }
+    if _VIEW_SET.get("map") is not None:
+        options["_view_set"] = _VIEW_SET["map"]
     if _CAMERA.get("cam") is not None:
         options["_camera"] = _CAMERA["cam"]
     if _CAMERA.get("grad"):
@@ -512,6 +528,67 @@ def mvpraymarch(
 
 _PLANES = {}
 _CAMERA = {}     # "cam": the camera of a mvpraymarch_camera call (rays generated in the kernels); "grad": camera_grad=True
+_VIEW_SET = {}   # "map": the view -> primitive set map of a mvpraymarch_sets call (or of view_set= elsewhere), or None
+
+
+@contextlib.contextmanager
+def _view_set_block(view_set):
+    """Raymarch calls within the block render view n from primitive set view_set[n] (see `mvpraymarch_sets`); None: as usual."""
+    prev = _VIEW_SET.get("map")
+    _VIEW_SET["map"] = view_set
+    try:
+        yield
+    finally:
+        _VIEW_SET["map"] = prev
+
+
+def _view_set_tensor(view_set, N, S, dev):
+    """The view -> set map as a private int32 [N] tensor on `dev`, for S primitive sets.  A map given on the host (a sequence of ints
+    or a CPU tensor) is range-checked here and raises ValueError; a CUDA map is not read back (no synchronisation): its entries
+    outside [0, S) make their views render empty, as the library defines it (int64 entries are clamped to [-1, S] first, so that
+    none wraps into range in the int32 conversion)."""
+    if not torch.is_tensor(view_set):
+        vals = list(view_set) if isinstance(view_set, (list, tuple, range)) else None
+        if vals is None or not all(isinstance(v, numbers.Integral) and not isinstance(v, bool) for v in vals):
+            raise TypeError("view_set must be an integer tensor or a sequence of ints, got %r" % (view_set,))
+        view_set = torch.tensor([int(v) for v in vals], dtype=torch.int64)
+    if view_set.dtype not in (torch.int32, torch.int64):
+        raise TypeError("view_set must be int32 or int64, got %s" % view_set.dtype)
+    if tuple(view_set.shape) != (N,):
+        raise ValueError("view_set must have shape [N] = [%d], got %s" % (N, list(view_set.shape)))
+    if not 1 <= S <= N:
+        raise ValueError("with view_set, the primitive batch (%d sets) must lie in [1, N] = [1, %d]" % (S, N))
+    if view_set.is_cuda:
+        if view_set.device != dev:
+            raise ValueError("view_set is on %s, the primitives on %s" % (view_set.device, dev))
+        return view_set.clamp(-1, S).to(torch.int32).contiguous()
+    if view_set.device.type != "cpu":
+        raise ValueError("view_set must be on the CPU or on the primitives' device, got %s" % view_set.device)
+    lo, hi = int(view_set.min()), int(view_set.max())
+    if lo < 0 or hi >= S:
+        raise ValueError("view_set entries must lie in [0, %d) (the primitive sets), got [%d, %d]" % (S, lo, hi))
+    return view_set.to(dtype=torch.int32).to(dev)
+
+
+def mvpraymarch_sets(raypos, raydir, stepsize, tminmax, primtransf, template, warp, view_set, planes=False, template_grad_dtype=None,
+                     **kwargs):
+    """`mvpraymarch` over S primitive sets -- S subjects, or S frames -- rendered in one launch, view n from set view_set[n]: the
+    primitives (primtransf, template, warp) are [S,K,...] with 1 <= S <= N, and so are their gradients (the template's in its dtype,
+    or fp32 per `template_grad_dtype`).  Each set's gradient sums those of its views; a set no view shows gets zero gradients.
+    view_set is an integer tensor [N] (int32 or int64, on the CPU or on the primitives' device) or a sequence of ints, and gets no
+    gradient.  A host map is range-checked (ValueError); a CUDA map is not read back, and a view whose entry is outside [0, S)
+    renders empty (zero colour and alpha) and contributes no gradient.  Replaces `payload.expand_views` + `mvpraymarch` +
+    `sum_views` for views that share a subject: no per-view copy of the primitives and no per-view gradient.  With usebvh=True each
+    set is marched in its own Morton order.  The other keyword arguments are those of `mvpraymarch`; ray gradients (camera fitting)
+    come through `mvpraymarch_camera(..., view_set=...)`.
+    Returns rayrgba [N,H,W,4], or (rayrgb [N,3,H,W], rayalpha [N,1,H,W]) with planes=True."""
+    if view_set is None:
+        raise TypeError("mvpraymarch_sets: view_set is required (use mvpraymarch for per-view or shared primitives)")
+    march = mvpraymarch_planes if planes else mvpraymarch
+    grad_block = _template_grad_block(template_grad_dtype) if _check_template_grad_dtype(template_grad_dtype) is not None \
+        else contextlib.nullcontext()
+    with grad_block, _view_set_block(view_set):
+        return march(raypos, raydir, stepsize, tminmax, primtransf, template, warp, **kwargs)
 
 
 def mvpraymarch_planes(*args, **kwargs):
@@ -525,7 +602,7 @@ def mvpraymarch_planes(*args, **kwargs):
 
 
 def mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, volradius, stepsize, primtransf, template, warp, planes=False,
-                       camera_grad=False, template_grad_dtype=None, **kwargs):
+                       camera_grad=False, template_grad_dtype=None, view_set=None, **kwargs):
     """`compute_raydirs` + `mvpraymarch` of models/autoencoder.py:240-252 as ONE call: the first six parameters are those of the
     reference's compute_raydirs (extensions/utils/utils.py:48-51), the rest those of `mvpraymarch` after its ray arguments.
 
@@ -542,7 +619,12 @@ def mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, volradius,
     avatar) it computes the ray gradients alone, with no template-sized gradient buffer and no payload-gradient scatter.
     template_grad_dtype=torch.float32 accumulates a bfloat16 template's gradient in fp32 (see the `template_grad_dtype` context
     manager); None leaves the setting of an enclosing `template_grad_dtype` block, by default the template's own dtype.
+    view_set: the views render S primitive sets [S,K,...], view n set view_set[n] (see `mvpraymarch_sets`).
     Returns rayrgba [N,H,W,4], or (rayrgb [N,3,H,W], rayalpha [N,1,H,W]) with planes=True."""
+    if view_set is not None:
+        with _view_set_block(view_set):
+            return mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, volradius, stepsize, primtransf, template, warp,
+                                      planes=planes, camera_grad=camera_grad, template_grad_dtype=template_grad_dtype, **kwargs)
     if _check_template_grad_dtype(template_grad_dtype) is not None:
         with _template_grad_block(template_grad_dtype):
             return mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, volradius, stepsize, primtransf, template, warp,

@@ -7,7 +7,7 @@ import contextlib
 import torch.nn as nn
 
 from .composite import split_rgba
-from .op import _check_template_grad_dtype, mvpraymarch, mvpraymarch_camera, mvpraymarch_planes, template_grad_dtype
+from .op import _check_template_grad_dtype, _view_set_block, mvpraymarch, mvpraymarch_camera, mvpraymarch_planes, template_grad_dtype
 
 
 class Raymarcher(nn.Module):
@@ -26,8 +26,10 @@ class Raymarcher(nn.Module):
     def _grad_dtype(self):
         return contextlib.nullcontext() if self.template_grad_dtype is None else template_grad_dtype(self.template_grad_dtype)
 
-    def forward(self, raypos, raydir, tminmax, decout, renderoptions={}, rayterm=None, with_pos_img=None):
-        with self._grad_dtype():
+    def forward(self, raypos, raydir, tminmax, decout, renderoptions={}, rayterm=None, with_pos_img=None, view_set=None):
+        """view_set: the decoder output holds S subjects' (or frames') primitives [S,K,...] and view n renders set view_set[n]
+        (see `op.mvpraymarch_sets`); None: one set per view, or one shared by all views."""
+        with self._grad_dtype(), _view_set_block(view_set):
             return self._forward(raypos, raydir, tminmax, decout, renderoptions, rayterm)
 
     def _forward(self, raypos, raydir, tminmax, decout, renderoptions, rayterm):
@@ -41,16 +43,18 @@ class Raymarcher(nn.Module):
         rayrgb, rayalpha = mvpraymarch_planes(*args, **kwargs)
         return rayrgb, rayalpha, None, None
 
-    def forward_camera(self, viewpos, viewrot, focal, princpt, pixelcoords, decout, renderoptions={}, rayterm=None, camera_grad=False):
+    def forward_camera(self, viewpos, viewrot, focal, princpt, pixelcoords, decout, renderoptions={}, rayterm=None, camera_grad=False,
+                       view_set=None):
         """`compute_raydirs(viewpos, viewrot, focal, princpt, pixelcoords, volradius)` followed by `forward(raypos, raydir, tminmax,
         ...)` -- models/autoencoder.py:240-252 -- as one call.  With `pixelcoords = (W, H)` the rays are generated inside the render
         kernels and never stored (`op.mvpraymarch_camera`); same return tuple as `forward`.  camera_grad=True: the camera tensors
-        that require grad get gradients (pose / calibration fitting through the image loss, see `op.mvpraymarch_camera`)."""
+        that require grad get gradients (pose / calibration fitting through the image loss, see `op.mvpraymarch_camera`).  view_set:
+        as in `forward`."""
         kwargs = dict(rayterm=rayterm, **{k: v for k, v in renderoptions.items() if k in mvpraymarch.__code__.co_varnames})
         out = mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, self.volume_radius, self.dt,
                                  (decout["primpos"], decout["primrot"], decout["primscale"]), decout["template"],
                                  decout["warp"] if "warp" in decout else None, planes=not self.with_rgba, camera_grad=camera_grad,
-                                 template_grad_dtype=self.template_grad_dtype, **kwargs)
+                                 template_grad_dtype=self.template_grad_dtype, view_set=view_set, **kwargs)
         if self.with_rgba:
             rayrgb, rayalpha = split_rgba(out)
             return rayrgb, rayalpha, out.permute(0, 3, 1, 2), None

@@ -227,6 +227,24 @@ int mvp_raymarch_backward(const mvp_backward_args *args, void *stream);
 int mvp_raymarch_backward_rays(const mvp_backward_args *args, float *grad_raypos, float *grad_raydir, float *grad_tminmax,
                                void *stream);
 
+/* Several subjects' (or frames') views in one launch.  view_set: device int32 [N]; view n renders primitive set view_set[n] of
+ * nsets, 1 <= nsets <= N.  primpos / primrot / primscale / tplate / warp, `order` and every gradient and clear_grad_* buffer then
+ * have a leading dimension of nsets instead of N ([nsets,K,...]); the gradients of all views of a set accumulate into that set, and
+ * a set that no view references gets zero gradients.  Every flag composes as in mvp_raymarch_forward / mvp_raymarch_backward(_rays),
+ * except MVP_FLAG_SHARED_PRIMS (the one-set form is nsets = 1 with an all-zero map): with it the call returns MVP_ERR_SHAPE.
+ * The map is input from outside the program and is not range-checked on the host: a view whose entry is outside [0, nsets) renders
+ * empty (zero colour and alpha, raysat unset), contributes no gradient and gets zero ray gradients; nothing is read or written out
+ * of bounds, and the other views are unaffected.  A workspace filled by a sets forward is valid (MVP_FLAG_ACCEL_VALID) only for a
+ * sets backward with the same map.  Argument errors are returned before any device work: view_set NULL is MVP_ERR_NULL, nsets
+ * outside [1, N] MVP_ERR_SHAPE, a view_set that is not 4-byte aligned MVP_ERR_ALIGN.
+ * The backward computes the ray gradients of mvp_raymarch_backward_rays when all three ray pointers are non-NULL and none when all
+ * three are NULL; any other combination is MVP_ERR_NULL.  mvp_workspace_bytes is unchanged (its per-slab records are sized N * K).
+ * mvp_build_accel / mvp_build_accel_camera have no sets form: a sets call builds its acceleration structure itself.
+ * The library supports these iff mvp_build_config() lists VIEW_SETS=1. */
+int mvp_raymarch_forward_sets(const mvp_forward_args *args, const int32_t *view_set, int32_t nsets, void *stream);
+int mvp_raymarch_backward_sets(const mvp_backward_args *args, const int32_t *view_set, int32_t nsets,
+                               float *grad_raypos, float *grad_raydir, float *grad_tminmax, void *stream);
+
 /* Pinhole ray generation + unit-cube clip (reference: extensions/utils/utils_kernel.cu:12-52).
  * viewpos [N,3], viewrot [N,3,3], focal [N,2], princpt [N,2], pixelcoords [N,H,W,2] or NULL (integer grid);
  * outputs raypos, raydir [N,H,W,3], tminmax [N,H,W,2]. */
