@@ -417,6 +417,52 @@ __global__ void __launch_bounds__(128) cam_params_kernel(int N, const float *__r
     bad[n] = ok ? 0 : 1;          // a degenerate camera (focal 0, non-finite) falls back to "every slab is a candidate", like a failed fit
 }
 
+// 1c. Pixels calls (mvp_raymarch_forward_pixels): the camera's rays at the sample positions pixelcoords[n,h,w] instead of (w, h).  The
+//     slab rectangles are in grid coordinates (w, h), so a view whose positions follow an axis-aligned affine map px = ox + sx w,
+//     py = oy + sy h -- the full grid, a crop, a stride, pixel centres at +0.5 -- gets the map folded into its camera record, which
+//     then projects straight to (w, h).  The map comes from three corners and is verified on every position (8 B read per ray) to
+//     within 0.05 of a grid step: a position off the map by d steps moves its ray's footprint by d steps, and the rectangles' margin
+//     is one step -- the tolerance and the margin of the ray-field fit (fit_camera_kernel).  A view that fails, or whose map is
+//     degenerate or not finite, is flagged in bad[], so every slab is a candidate on it, as after a failed fit.  Runs after
+//     cam_params_kernel; block 0 of a view rewrites its record.
+__global__ void __launch_bounds__(kFitThreads) pix_map_kernel(int H, int W, const float2 *__restrict__ pix, Cam *cam, int *bad) {
+    const int n = blockIdx.y;
+    const size_t HW = (size_t)H * W;
+    const float2 *pc = pix + (size_t)n * HW;
+    const float2 c00 = __ldg(pc), c10 = __ldg(pc + (W - 1)), c01 = __ldg(pc + (size_t)(H - 1) * W);
+    const float ox = c00.x, oy = c00.y;
+    const float sx = W > 1 ? __fdiv_rn(__fsub_rn(c10.x, ox), (float)(W - 1)) : 1.f;
+    const float sy = H > 1 ? __fdiv_rn(__fsub_rn(c01.y, oy), (float)(H - 1)) : 1.f;
+    const bool ok = isfinite(ox) && isfinite(oy) && isfinite(sx) && isfinite(sy) && sx != 0.f && sy != 0.f;
+    int fail = !ok;
+    if (ok) {
+        const float tx = 0.05f * fabsf(sx), ty = 0.05f * fabsf(sy);
+        const size_t base = (size_t)blockIdx.x * (kFitThreads * kFitRaysPerThread);
+#pragma unroll
+        for (int it = 0; it < kFitRaysPerThread; ++it) {
+            const size_t r = base + (size_t)it * kFitThreads + threadIdx.x;
+            if (r < HW) {
+                const float2 q = __ldg(pc + r);
+                const float w = (float)(int)(r % (size_t)W), h = (float)(int)(r / (size_t)W);
+                fail |= !(fabsf(__fsub_rn(q.x, __fmaf_rn(sx, w, ox))) < tx && fabsf(__fsub_rn(q.y, __fmaf_rn(sy, h, oy))) < ty);
+            }
+        }
+    }
+    fail = __syncthreads_or(fail);
+    if (threadIdx.x == 0) {
+        if (fail) atomicOr(bad + n, 1);
+        if (blockIdx.x == 0 && ok) {
+            // pixel (px, py, 1) ~ minv (P - o), so (w, h, 1) ~ ((row0 - ox row2) / sx, (row1 - oy row2) / sy, row2) (P - o)
+            Cam c = cam[n];
+            for (int i = 0; i < 3; ++i) {
+                c.minv[i] = (float)(((double)c.minv[i] - (double)ox * (double)c.minv[6 + i]) / (double)sx);
+                c.minv[3 + i] = (float)(((double)c.minv[3 + i] - (double)oy * (double)c.minv[6 + i]) / (double)sy);
+            }
+            cam[n] = c;
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------------------
 // 2. per-slab record + pixel rectangle
 //    record (4 x float4): (pos.xyz, s.x) (R row0, s.y) (R row1, s.z) (R row2, 0)
@@ -1034,11 +1080,13 @@ __device__ __forceinline__ void mbar_wait(unsigned long long *bar, unsigned pari
 #endif
 
 // This lane's ray: read from the caller's ray tensors, or -- mvp_camera -- generated from the view's camera record with the arithmetic
-// of mvp_compute_raydirs (raygen.h; utils_kernel.cu:32-46), in which case raypos / raydir / tminmax are never touched.
+// of mvp_compute_raydirs (raygen.h; utils_kernel.cu:32-46), in which case raypos / raydir / tminmax are never touched.  kPix: the
+// camera form at the sample position pixelcoords[r] (8 bytes read) instead of the integer pixel (cx, cy).
+template <bool kPix = false>
 __device__ __forceinline__ Ray fetch_ray(const float *__restrict__ raypos, const float *__restrict__ raydir, const float *__restrict__ tminmax,
-                                         const float4 *__restrict__ raycam, int n, size_t r, int cx, int cy) {
+                                         const float4 *__restrict__ raycam, const float2 *__restrict__ pix, int n, size_t r, int cx, int cy) {
     Ray ray;
-    if (raycam) {
+    if (kPix || raycam) {
         const float4 q0 = __ldg(raycam + (size_t)n * 4), q1 = __ldg(raycam + (size_t)n * 4 + 1), q2 = __ldg(raycam + (size_t)n * 4 + 2),
                      q3 = __ldg(raycam + (size_t)n * 4 + 3);
         MvpRayCam c;
@@ -1046,7 +1094,8 @@ __device__ __forceinline__ Ray fetch_ray(const float *__restrict__ raypos, const
         c.R[0] = q0.w; c.R[1] = q1.x; c.R[2] = q1.y; c.R[3] = q1.z; c.R[4] = q1.w; c.R[5] = q2.x; c.R[6] = q2.y; c.R[7] = q2.z; c.R[8] = q2.w;
         c.pcx = q3.x; c.pcy = q3.y; c.fx = q3.z; c.fy = q3.w;
         ray.ox = c.ox; ray.oy = c.oy; ray.oz = c.oz;
-        mvp_gen_ray(c, (float)cx, (float)cy, ray.dx, ray.dy, ray.dz, ray.tmin, ray.tmax);
+        const float2 pc = kPix ? __ldg(pix + r) : make_float2((float)cx, (float)cy);
+        mvp_gen_ray(c, pc.x, pc.y, ray.dx, ray.dy, ray.dz, ray.tmin, ray.tmax);
     } else {
         ray.ox = __ldg(raypos + r * 3 + 0); ray.oy = __ldg(raypos + r * 3 + 1); ray.oz = __ldg(raypos + r * 3 + 2);
         ray.dx = __ldg(raydir + r * 3 + 0); ray.dy = __ldg(raydir + r * 3 + 1); ray.dz = __ldg(raydir + r * 3 + 2);
@@ -1126,12 +1175,15 @@ struct Params {
     // sets calls (kSets kernels only): view n renders primitive set vset[n] of nsets, see checked_set
     const int *vset;
     int nsets;
+    // pixels calls (kPix kernels only): [N,H,W,2] sample positions of the camera's rays, see fetch_ray
+    const float2 *pix;
 };
 
-// Index of view n's primitive set: n (per-view tensors), 0 (MVP_FLAG_SHARED_PRIMS) or, in the kSets kernels, its checked map entry
-template <bool kSets>
+// Index of view n's primitive set: n (per-view tensors), 0 (MVP_FLAG_SHARED_PRIMS) or, in the kSets kernels, its checked map entry.
+// The pixels calls have kSets kernels only, which serve calls without a map (p.vset NULL) as well.
+template <bool kSets, bool kPix = false>
 __device__ __forceinline__ int prim_set(const Params &p, int n) {
-    if (kSets) return checked_set(p.vset, p.nsets, n);
+    if (kSets && (!kPix || p.vset)) return checked_set(p.vset, p.nsets, n);
     return n * p.pview;
 }
 
@@ -1162,7 +1214,7 @@ __device__ __forceinline__ bool tile_bucket_empty(const Params &p, int n, int tx
 // "every lane starts at its own first hit" (the reference's lock-step loop) and over a plane fitted to the first-hit
 // depths because neighbouring slabs sit at randomly different depths while the sweep planes stay coherent.
 // Returns false when the list would exceed CAP (< 512): the caller hands the tile to the 512-entry kernel.
-template <int CAP, bool kPrefetch, bool kSets>
+template <int CAP, bool kPrefetch, bool kSets, bool kPix = false>
 __device__ __forceinline__ bool build_tile_list(const Params &p, float rdt, int n, int tx, int ty, int lane, TileCtx &c,
                                                 int *s_k, int *s_iv, RowEntry *s_stage, unsigned long long *s_bar, float &t,
                                                 float &x, float &y, float &z, float &r1e, int &j0) {
@@ -1170,7 +1222,7 @@ __device__ __forceinline__ bool build_tile_list(const Params &p, float rdt, int 
     c.inimg = (px < p.W) && (py < p.H);
     const int cx = min(px, p.W - 1), cy = min(py, p.H - 1);
     const size_t r = ((size_t)n * p.H + cy) * p.W + cx;
-    c.ray = fetch_ray(p.raypos, p.raydir, p.tminmax, p.raycam, n, r, cx, cy);
+    c.ray = fetch_ray<kPix>(p.raypos, p.raydir, p.tminmax, p.raycam, p.pix, n, r, cx, cy);
     c.rt0 = CUDART_INF_F; c.rt1 = -CUDART_INF_F;
 
     const float tsteps = c.ray.tmin * rdt;            // lattice origin of this lane, in steps
@@ -1184,7 +1236,7 @@ __device__ __forceinline__ bool build_tile_list(const Params &p, float rdt, int 
     march_margins(c.ray, rdt, epos, eps0);
 #endif
 
-    const float4 *packn = p.pack + (size_t)prim_set<kSets>(p, n) * p.K * 4;
+    const float4 *packn = p.pack + (size_t)prim_set<kSets, kPix>(p, n) * p.K * 4;
     const int cnt = p.rowcnt[(size_t)n * p.R + ty];
     const bool overflow = cnt > p.rowcap;
 #if MVP_XBUCKETS
@@ -1234,7 +1286,7 @@ __device__ __forceinline__ bool build_tile_list(const Params &p, float rdt, int 
                 k = e.k; xr = e.xr;
                 cand = true;
             } else {
-                k = slab_at_rank(p.order ? p.order + (size_t)prim_set<kSets>(p, n) * p.K : nullptr, p.K, kstart, idx);
+                k = slab_at_rank(p.order ? p.order + (size_t)prim_set<kSets, kPix>(p, n) * p.K : nullptr, p.K, kstart, idx);
                 xr = __ldg(rxn + k);
                 unsigned yr = __ldg(ryn + k);
                 int y0 = (int)(yr & 0xffffu), y1 = (int)(yr >> 16);
@@ -1302,7 +1354,7 @@ __device__ __forceinline__ bool build_tile_list(const Params &p, float rdt, int 
     // TMA bulk prefetch (cp.async.bulk.prefetch.L2): pull the payload slabs this tile is about to sample into L2 while
     // the lattice set-up runs; one lane per slab, fire and forget.
     if (kPrefetch && p.slab_bytes >= 16) {
-        const char *tp = reinterpret_cast<const char *>(p.tplate) + (size_t)prim_set<kSets>(p, n) * p.K * p.slab_bytes;
+        const char *tp = reinterpret_cast<const char *>(p.tplate) + (size_t)prim_set<kSets, kPix>(p, n) * p.K * p.slab_bytes;
         for (int i = lane; i < nl; i += 32) {
             const char *a = tp + (size_t)s_k[i] * p.slab_bytes;
             asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(a), "r"(p.slab_bytes) : "memory");
@@ -1349,7 +1401,7 @@ __device__ __forceinline__ void save_tile_list(const Params &p, int n, int tx, i
 // Backward: restore the outputs of build_tile_list the adjoint uses (ray, off, list, first step and its position) from
 // what the forward saved.  Returns (warp-uniform) 1 = loaded, 0 = this tile's list was not saved (rebuild it), 2 = it was
 // saved but is longer than this kernel's shared-memory list (the 512-entry kernel takes the tile).
-template <int CAP>
+template <int CAP, bool kPix = false>
 __device__ __forceinline__ int load_saved_tile_list(const Params &p, float rdt, int n, int tx, int ty, int lane, TileCtx &c, int *s_k,
                                                      int *s_iv, float &x, float &y, float &z, int &j0) {
     const int2 hdr = __ldg(p.tilehdr + ((size_t)n * p.TYn + ty) * p.TXn + tx);
@@ -1363,7 +1415,7 @@ __device__ __forceinline__ int load_saved_tile_list(const Params &p, float rdt, 
     c.inimg = (px < p.W) && (py < p.H);
     const int cx = min(px, p.W - 1), cy = min(py, p.H - 1);
     const size_t r = ((size_t)n * p.H + cy) * p.W + cx;
-    c.ray = fetch_ray(p.raypos, p.raydir, p.tminmax, p.raycam, n, r, cx, cy);
+    c.ray = fetch_ray<kPix>(p.raypos, p.raydir, p.tminmax, p.raycam, p.pix, n, r, cx, cy);
     const float tsteps = c.ray.tmin * rdt;
     float tref = c.inimg ? tsteps : CUDART_INF_F;
 #pragma unroll
@@ -1608,7 +1660,7 @@ struct __align__(16) FwdWarpSmem {   // per-warp shared state of the forward ker
 //    fits (almost all) with a small shared-memory footprint (more L1 for the voxel gathers) and flags the rest;
 //    the CAP == 512 variant then renders only the flagged tiles.
 // ------------------------------------------------------------------------------------------------------
-template <int T, bool kGrad, int CAP, bool kWarp, typename V, bool kSets>
+template <int T, bool kGrad, int CAP, bool kWarp, typename V, bool kSets, bool kPix>
 __device__ __forceinline__ bool forward_tile(const Params &p, const int n, const int tx, const int ty, const int lane, FwdWarpSmem<CAP, kGrad> *const S) {
     // all per-warp shared state lives in one record: every address below is (one pinned per-warp base) + immediate
     int *const sk = S->k, *const siv = S->iv, *const rm = S->rm;
@@ -1647,7 +1699,7 @@ __device__ __forceinline__ bool forward_tile(const Params &p, const int n, const
     TileCtx c;
     float t, x, y, z, r1e;
     int j0;
-    if (!build_tile_list<CAP, true, kSets>(p, rdt, n, tx, ty, lane, c, sk, siv, sstage, sbar, t, x, y, z, r1e, j0)) return false;
+    if (!build_tile_list<CAP, true, kSets, kPix>(p, rdt, n, tx, ty, lane, c, sk, siv, sstage, sbar, t, x, y, z, r1e, j0)) return false;
 
     const int px = tx * kTileW + (lane & 7), py = ty * kTileH + (lane >> 3);
     const size_t r = ((size_t)n * p.H + min(py, p.H - 1)) * p.W + min(px, p.W - 1);
@@ -1675,11 +1727,11 @@ __device__ __forceinline__ bool forward_tile(const Params &p, const int n, const
     if (nl > 192) MVP_STAT2(7, 1);
 #endif
     const int nwords = (nl + 31) >> 5;
-    const float4 *packn = p.pack + (size_t)prim_set<kSets>(p, n) * p.K * 4;
+    const float4 *packn = p.pack + (size_t)prim_set<kSets, kPix>(p, n) * p.K * 4;
     // voxels per slab: a compile-time constant for the cubic 8^3 / 16^3 specialisations, so that a slab's address is a shift and an add
     // wherever the register cap makes the compiler re-derive it (it was ~30 of the 159 instructions of a batch gather)
     const size_t slabsz = T > 0 ? (size_t)(T * T * T) : (size_t)p.TD * p.TH * p.TW;
-    const V *tpn = reinterpret_cast<const V *>(p.tplate) + (size_t)prim_set<kSets>(p, n) * p.K * slabsz;
+    const V *tpn = reinterpret_cast<const V *>(p.tplate) + (size_t)prim_set<kSets, kPix>(p, n) * p.K * slabsz;
     const int kstart = dfs_kstart(p.K);
     {
         // pinned: under the register cap the compiler would otherwise re-materialise this base address per event
@@ -1717,7 +1769,7 @@ __device__ __forceinline__ bool forward_tile(const Params &p, const int n, const
                     sat = true;
                     if (kGrad) {
                         jsat = rm[b] + c.off;
-                        ranksat = rank_of_slab(p.rankof ? p.rankof + (size_t)prim_set<kSets>(p, n) * p.K : nullptr, p.K, kstart, sk[(__float_as_int(rr.w) >> 5) & 1023]);
+                        ranksat = rank_of_slab(p.rankof ? p.rankof + (size_t)prim_set<kSets, kPix>(p, n) * p.K : nullptr, p.K, kstart, sk[(__float_as_int(rr.w) >> 5) & 1023]);
                         abefore = acc.w;
                     }
                 }
@@ -1733,7 +1785,7 @@ __device__ __forceinline__ bool forward_tile(const Params &p, const int n, const
         float4 sres = make_float4(0.f, 0.f, 0.f, 0.f);
         if (act) {
             const int kk = sk[(__float_as_int(rec.w) >> 5) & 1023];
-            if (kWarp) sres = sample_slab_warped(tpn + (size_t)kk * slabsz, p.warp + ((size_t)prim_set<kSets>(p, n) * p.K + kk) * ((size_t)p.WD * p.WH * p.WW * 3), rec.x, rec.y, rec.z, p);
+            if (kWarp) sres = sample_slab_warped(tpn + (size_t)kk * slabsz, p.warp + ((size_t)prim_set<kSets, kPix>(p, n) * p.K + kk) * ((size_t)p.WD * p.WH * p.WW * 3), rec.x, rec.y, rec.z, p);
             else sres = sample_slab<T, V>(tpn + (size_t)kk * slabsz, rec.x, rec.y, rec.z, p.TD, p.TH, p.TW, p.fadescale, p.fadeexp);
         }
         __syncwarp();
@@ -1909,8 +1961,9 @@ __device__ __forceinline__ void clear_grad_slices(const Params &p, size_t g, int
     }
 }
 
-// kSets: a sets call (mvp_raymarch_forward_sets), the primitive set of a view from its map entry (prim_set)
-template <int T, bool kGrad, int CAP, bool kWarp, typename V, bool kSets = false>
+// kSets: a sets call (mvp_raymarch_forward_sets), the primitive set of a view from its map entry (prim_set).  kPix: a pixels call
+// (mvp_raymarch_forward_pixels), the camera's rays at the caller's sample positions (fetch_ray)
+template <int T, bool kGrad, int CAP, bool kWarp, typename V, bool kSets = false, bool kPix = false>
 __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_FWD_MINB * 4) / kWarps : 16 / kWarps) render_forward_kernel(const Params p) {
     __shared__ FwdWarpSmem<CAP, kGrad> s_w[kWarps];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -1921,7 +1974,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         for (int i = blockIdx.x * kWarps + warp; i < cnt; i += gridDim.x * kWarps) {
             const int id = p.heavylist[i];
             const int tx = id % p.TXn, ty = (id / p.TXn) % p.TYn, n = id / (p.TXn * p.TYn);
-            forward_tile<T, kGrad, CAP, kWarp, V, kSets>(p, n, tx, ty, lane, S);
+            forward_tile<T, kGrad, CAP, kWarp, V, kSets, kPix>(p, n, tx, ty, lane, S);
             __syncwarp();
         }
     } else {
@@ -1940,7 +1993,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         long long g0_;
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g0_));
 #endif
-        if (!forward_tile<T, kGrad, CAP, kWarp, V, kSets>(p, n, tx, ty, lane, S) && lane == 0)
+        if (!forward_tile<T, kGrad, CAP, kWarp, V, kSets, kPix>(p, n, tx, ty, lane, S) && lane == 0)
             p.heavylist[atomicAdd(p.heavycnt, 1)] = (n * p.TYn + ty) * p.TXn + tx;
 #if MVP_TILE_CLOCKS
         if (lane == 0) {
@@ -2082,7 +2135,7 @@ constexpr int kGradAll = 0;         // transforms, template (+ warp field)
 constexpr int kGradNoPayload = 1;   // transforms only (MVP_FLAG_NO_TPLATE_GRAD): no payload-gradient scatter
 constexpr int kGradRaysOnly = 2;    // ray gradients only (MVP_FLAG_RAY_GRADS_ONLY; kRayGrad kernels): no transform sums either
 
-template <int T, int CAP, bool kWarp, typename V, bool kRayGrad, int kSet, bool kSets>
+template <int T, int CAP, bool kWarp, typename V, bool kRayGrad, int kSet, bool kSets, bool kPix>
 __device__ __forceinline__ bool backward_tile(const Params &p, const int n, const int tx, const int ty, const int lane, BwdWarpSmem<CAP> *const S) {
     static_assert(kSet != kGradRaysOnly || kRayGrad, "a rays-only backward computes the ray gradients");
     int *const sk = S->k, *const siv = S->iv;
@@ -2099,10 +2152,10 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
     int j0;
     int have = 0;           // 0: rebuild the list, 1: loaded what the forward saved, 2: the saved list does not fit this kernel
 #if MVP_LIST_REUSE
-    have = load_saved_tile_list<CAP>(p, rdt, n, tx, ty, lane, c, sk, siv, xb, yb, zb, j0);
+    have = load_saved_tile_list<CAP, kPix>(p, rdt, n, tx, ty, lane, c, sk, siv, xb, yb, zb, j0);
     if (have == 2) return false;
 #endif
-    if (have == 0 && !build_tile_list<CAP, false, kSets>(p, rdt, n, tx, ty, lane, c, sk, siv, sstage, sbar, t0, xb, yb, zb, r1e, j0)) return false;
+    if (have == 0 && !build_tile_list<CAP, false, kSets, kPix>(p, rdt, n, tx, ty, lane, c, sk, siv, sstage, sbar, t0, xb, yb, zb, r1e, j0)) return false;
     const int nl = c.nl;
     if (nl == 0) {
         if (kRayGrad) store_ray_grads(p, n, tx, ty, lane, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f);
@@ -2151,11 +2204,11 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
         return true;
     }
 
-    const float4 *packn = p.pack + (size_t)prim_set<kSets>(p, n) * p.K * 4;
+    const float4 *packn = p.pack + (size_t)prim_set<kSets, kPix>(p, n) * p.K * 4;
     const size_t slabsz = (size_t)p.TD * p.TH * p.TW;   // (a compile-time T^3 here makes the compiler keep slab addresses in registers: 64 B of spills)
     // bases of the primitive tensors are re-derived from the parameter block where they are used (cheap constant-bank
     // arithmetic) instead of living in a dozen registers for the whole tile
-    const size_t pvK = (size_t)prim_set<kSets>(p, n) * p.K;
+    const size_t pvK = (size_t)prim_set<kSets, kPix>(p, n) * p.K;
     const int td = T > 0 ? T : p.TD, th = T > 0 ? T : p.TH, tw = T > 0 ? T : p.TW;
     const float gmx = (float)(tw - 1) * 0.5f, gmy = (float)(th - 1) * 0.5f, gmz = (float)(td - 1) * 0.5f;
     const int sx = tw > 1 ? 1 : 0, sy = th > 1 ? tw : 0, sz = td > 1 ? th * tw : 0;
@@ -2224,7 +2277,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                 word &= word - 1;
                 const int slot = w * 32 + bit;
                 const int k = sk[slot];
-                const int rank = rank_of_slab(p.rankof ? p.rankof + (size_t)prim_set<kSets>(p, n) * p.K : nullptr, p.K, kstart, k);
+                const int rank = rank_of_slab(p.rankof ? p.rankof + (size_t)prim_set<kSets, kPix>(p, n) * p.K : nullptr, p.K, kstart, k);
 #if MVP_BWD_SMEMREC
                 __syncwarp();                                  // the previous slab's last readers of the record are done
                 if (lane < 4) S->rec[lane] = __ldg(packn + (size_t)k * 4 + lane);
@@ -2512,8 +2565,8 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         } else {
                         // ---- algo 1 (PrimSamplerTW<true>): payload sampled at the warp-field-displaced position ----
                         const size_t wsl = (size_t)p.WD * p.WH * p.WW * 3;
-                        const float *wk = p.warp + ((size_t)prim_set<kSets>(p, n) * p.K + k) * wsl;
-                        float *gwk = kSet == kGradAll ? p.g_warp + ((size_t)prim_set<kSets>(p, n) * p.K + k) * wsl : nullptr;
+                        const float *wk = p.warp + ((size_t)prim_set<kSets, kPix>(p, n) * p.K + k) * wsl;
+                        float *gwk = kSet == kGradAll ? p.g_warp + ((size_t)prim_set<kSets, kPix>(p, n) * p.K + k) * wsl : nullptr;
                         const float e1 = p.fadeexp - 1.f;
                         const float pw0 = __powf(fabsf(y0), e1), pw1 = __powf(fabsf(y1), e1), pw2 = __powf(fabsf(y2), e1);
                         const float fade = __expf(-p.fadescale * (pw0 * fabsf(y0) + pw1 * fabsf(y1) + pw2 * fabsf(y2)));
@@ -2692,8 +2745,8 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
 
 // kRayGrad: also write the per-ray gradients p.g_raypos / g_raydir / g_tminmax (mvp_raymarch_backward_rays); false compiles to
 // the plain backward.  kSet: the gradient set (kGradAll, kGradNoPayload, kGradRaysOnly); the default is the full backward.  kSets: a
-// sets call (mvp_raymarch_backward_sets), as in render_forward_kernel.
-template <int T, int CAP, bool kWarp, typename V, bool kRayGrad = false, int kSet = kGradAll, bool kSets = false>
+// sets call (mvp_raymarch_backward_sets), as in render_forward_kernel; kPix: a pixels call (mvp_raymarch_backward_pixels), as there.
+template <int T, int CAP, bool kWarp, typename V, bool kRayGrad = false, int kSet = kGradAll, bool kSets = false, bool kPix = false>
 __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_BWD_MINB * 4) / kWarps : 12 / kWarps) render_backward_kernel(const Params p) {
     __shared__ typename BwdSmemOf<CAP, kRayGrad>::type s_w[kWarps];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -2703,7 +2756,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         for (int i = blockIdx.x * kWarps + warp; i < cnt; i += gridDim.x * kWarps) {
             const int id = p.heavylist[i];
             const int tx = id % p.TXn, ty = (id / p.TXn) % p.TYn, n = id / (p.TXn * p.TYn);
-            backward_tile<T, CAP, kWarp, V, kRayGrad, kSet, kSets>(p, n, tx, ty, lane, S);
+            backward_tile<T, CAP, kWarp, V, kRayGrad, kSet, kSets, kPix>(p, n, tx, ty, lane, S);
             __syncwarp();
         }
     } else {
@@ -2716,7 +2769,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         const int tx = blockIdx.x * kBlkTX + (warp % kBlkTX), ty = blockIdx.y * kBlkTY + (warp / kBlkTX), n = blockIdx.z;
 #endif
         if (tx >= p.TXn || ty >= p.TYn) return;
-        if (!backward_tile<T, CAP, kWarp, V, kRayGrad, kSet, kSets>(p, n, tx, ty, lane, S) && lane == 0)
+        if (!backward_tile<T, CAP, kWarp, V, kRayGrad, kSet, kSets, kPix>(p, n, tx, ty, lane, S) && lane == 0)
             p.heavylist[atomicAdd(p.heavycnt, 1)] = (n * p.TYn + ty) * p.TXn + tx;
     }
 }
@@ -2772,10 +2825,11 @@ int check_shape(const mvp_shape &s) {
     return MVP_OK;
 }
 
-// camera: NULL or a checked mvp_camera (then raypos / raydir are not used); vset: NULL, or the view -> set map of a sets call
-// (then pview is ignored, and the primitive tensors and order hold nsets sets)
+// camera: NULL or a checked mvp_camera (then raypos / raydir are not used); pix: NULL, or with a camera the sample positions of a
+// pixels call; vset: NULL, or the view -> set map of a sets call (then pview is ignored, and the primitive tensors and order hold
+// nsets sets)
 int launch_accel(const mvp_shape &s, int pview, const int *vset, int nsets, const int *order, const float *raypos, const float *raydir,
-                 const mvp_camera *camera, const float *primpos, const float *primrot, const float *primscale, char *ws, const Layout &L,
+                 const mvp_camera *camera, const float2 *pix, const float *primpos, const float *primrot, const float *primscale, char *ws, const Layout &L,
                  cudaStream_t st) {
     const int ostride = pview ? s.K : 0;      // the order belongs to the primitives: one per view, or one shared by all views
     Cam *cam = reinterpret_cast<Cam *>(ws + L.cam);
@@ -2798,6 +2852,7 @@ int launch_accel(const mvp_shape &s, int pview, const int *vset, int nsets, cons
                    camera->princpt, camera->volradius, cam, bad, reinterpret_cast<float4 *>(ws + L.raycam));
     else
         MVP_LAUNCH(fit_camera_kernel, gfit, kFitThreads, 0, st, s.H, s.W, raypos, raydir, cam, bad);
+    if (pix) MVP_LAUNCH(pix_map_kernel, gfit, kFitThreads, 0, st, s.H, s.W, pix, cam, bad);
     const size_t NK = (size_t)s.N * s.K;
     MVP_LAUNCH(prim_setup_kernel, (unsigned)((NK + 127) / 128), 128, 0, st, s.N, s.K, s.H, s.W, pview, vset, nsets, primpos, primrot, primscale, cam, bad,
                reinterpret_cast<float4 *>(ws + L.pack), reinterpret_cast<unsigned *>(ws + L.rx), reinterpret_cast<unsigned *>(ws + L.ry));
@@ -2834,6 +2889,7 @@ int launch_accel(const mvp_shape &s, int pview, const int *vset, int nsets, cons
                                                                          camera->volradius, cam, bad, reinterpret_cast<float4 *>(ws + L.raycam));
     else
         fit_camera_kernel<<<gfit, kFitThreads, 0, st>>>(s.H, s.W, raypos, raydir, cam, bad);
+    if (pix) pix_map_kernel<<<gfit, kFitThreads, 0, st>>>(s.H, s.W, pix, cam, bad);
     const size_t NK = (size_t)s.N * s.K;
     prim_setup_kernel<<<(unsigned)((NK + 127) / 128), 128, 0, st>>>(
         s.N, s.K, s.H, s.W, pview, vset, nsets, primpos, primrot, primscale, cam, bad, reinterpret_cast<float4 *>(ws + L.pack),
@@ -2940,7 +2996,7 @@ const char *mvp_build_config(void) {
     return "LIST_REUSE=" MVP_STR(MVP_LIST_REUSE)
            " LIST_MARGIN=" MVP_STR(MVP_LIST_MARGIN) " XBUCKETS=" MVP_STR(MVP_XBUCKETS) " FASTCAP=" MVP_STR(MVP_FWD_FASTCAP) "/" MVP_STR(MVP_BWD_FASTCAP) " SMEM_UNION=" MVP_STR(MVP_SMEM_UNION) " CARVEOUT=" MVP_STR(MVP_FWD_CARVEOUT) "/" MVP_STR(MVP_BWD_CARVEOUT) " FWD_RING=" MVP_STR(MVP_FWD_RING) " BWD_SMEMREC=" MVP_STR(MVP_BWD_SMEMREC) " BWD_LANESMEM=" MVP_STR(MVP_BWD_LANESMEM) " CTA_ORDER=" MVP_STR(MVP_CTA_ORDER) " CTA_ORDER_MIN=" MVP_STR(MVP_CTA_ORDER_MIN)
            " CHUNK=" MVP_STR(MVP_CHUNK) " FWD_MINB=" MVP_STR(MVP_FWD_MINB) " BWD_MINB=" MVP_STR(MVP_BWD_MINB)
-           " WARPS=" MVP_STR(MVP_WARPS) " BLK_TX=" MVP_STR(MVP_BLK_TX) " TPLATE_BF16=1 EPILOGUE_BF16=1 RAY_GRADS=1 GRAD_TPLATE_F32=1 GRAD_SELECT=1 VIEW_SETS=1"
+           " WARPS=" MVP_STR(MVP_WARPS) " BLK_TX=" MVP_STR(MVP_BLK_TX) " TPLATE_BF16=1 EPILOGUE_BF16=1 RAY_GRADS=1 GRAD_TPLATE_F32=1 GRAD_SELECT=1 VIEW_SETS=1 CAMERA_PIXELS=1"
 #ifdef MVP_CPU_EMUL
            " CPU_EMUL"
 #endif
@@ -2975,7 +3031,7 @@ int mvp_build_accel(const mvp_shape *shape, uint32_t flags, const int32_t *order
     if (rc != MVP_OK) return rc;
     const Layout L = make_layout(*shape);
     if (workspace_bytes < L.total || ((uintptr_t)workspace & 255)) return MVP_ERR_WORKSPACE;
-    return launch_accel(*shape, (flags & MVP_FLAG_SHARED_PRIMS) ? 0 : 1, nullptr, 0, order, raypos, raydir, nullptr, primpos, primrot, primscale,
+    return launch_accel(*shape, (flags & MVP_FLAG_SHARED_PRIMS) ? 0 : 1, nullptr, 0, order, raypos, raydir, nullptr, nullptr, primpos, primrot, primscale,
                         (char *)workspace, L, (cudaStream_t)stream);
 }
 
@@ -2998,7 +3054,7 @@ int mvp_build_accel_camera(const mvp_shape *shape, uint32_t flags, const int32_t
     if (rc <= 0) return rc == 0 ? MVP_ERR_NULL : rc;
     const Layout L = make_layout(*shape);
     if (workspace_bytes < L.total || ((uintptr_t)workspace & 255)) return MVP_ERR_WORKSPACE;
-    return launch_accel(*shape, (flags & MVP_FLAG_SHARED_PRIMS) ? 0 : 1, nullptr, 0, order, nullptr, nullptr, camera, primpos, primrot, primscale,
+    return launch_accel(*shape, (flags & MVP_FLAG_SHARED_PRIMS) ? 0 : 1, nullptr, 0, order, nullptr, nullptr, camera, nullptr, primpos, primrot, primscale,
                         (char *)workspace, L, (cudaStream_t)stream);
 }
 
@@ -3027,6 +3083,11 @@ size_t mvp_debug_heavy_offset(const mvp_shape *shape) {
     return make_layout(*shape).heavycnt;
 }
 
+size_t mvp_debug_view_fallback_offset(const mvp_shape *shape) {
+    if (!shape || check_shape(*shape) != MVP_OK) return 0;
+    return make_layout(*shape).bad;
+}
+
 int mvp_forward_launch_count(uint32_t flags) { return (flags & MVP_FLAG_ACCEL_VALID) ? 2 : 6; }   // + 2 ordering kernels for small launches
 int mvp_backward_launch_count(uint32_t flags) { return (flags & MVP_FLAG_ACCEL_VALID) ? 2 : 6; }
 
@@ -3049,11 +3110,13 @@ static int check_view_sets(const mvp_shape &s, uint32_t flags, const int32_t *vi
     return misaligned(view_set, 4) ? MVP_ERR_ALIGN : MVP_OK;
 }
 
-// mvp_raymarch_forward, and with vset != NULL mvp_raymarch_forward_sets (struct and map checked by the caller)
-static int forward_impl(const mvp_forward_args *a, const int32_t *vset, int nsets, void *stream) {
+// mvp_raymarch_forward, with vset != NULL mvp_raymarch_forward_sets (struct and map checked by the caller), with pix != NULL
+// mvp_raymarch_forward_pixels (the camera's rays at those sample positions)
+static int forward_impl(const mvp_forward_args *a, const int32_t *vset, int nsets, const float2 *pix, void *stream) {
     const int camrc = check_camera(a->camera);
     if (camrc < 0) return camrc;
     const mvp_camera *const camera = camrc ? &a->camera : nullptr;      // rays generated in the kernels: the ray tensors are not read
+    if (pix && !camera) return MVP_ERR_NULL;
     if ((!camera && (!a->raypos || !a->raydir || !a->tminmax)) || !a->primpos || !a->primrot || !a->primscale || !a->tplate || !a->workspace)
         return MVP_ERR_NULL;
     if ((a->rayrgb_nchw == nullptr) != (a->rayalpha_nchw == nullptr)) return MVP_ERR_NULL;
@@ -3079,13 +3142,13 @@ static int forward_impl(const mvp_forward_args *a, const int32_t *vset, int nset
         misaligned(a->primscale, 4) || misaligned(a->raysat, 4) || misaligned(a->warp, 4) || misaligned(a->rayrgb_nchw, 4) ||
         misaligned(a->rayalpha_nchw, 4) || misaligned(a->order, 4) || misaligned(clr_primpos, 16) ||
         misaligned(clr_primrot, 16) || misaligned(clr_primscale, 16) || misaligned(clr_tplate, 16) ||
-        misaligned(clr_warp, 16))
+        misaligned(clr_warp, 16) || misaligned(pix, 8))
         return MVP_ERR_ALIGN;
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)a->workspace;
     const int pview = (a->flags & MVP_FLAG_SHARED_PRIMS) ? 0 : 1;
     if (!(a->flags & MVP_FLAG_ACCEL_VALID)) {
-        rc = launch_accel(a->shape, pview, vset, nsets, a->order, a->raypos, a->raydir, camera, a->primpos, a->primrot, a->primscale, ws,
+        rc = launch_accel(a->shape, pview, vset, nsets, a->order, a->raypos, a->raydir, camera, pix, a->primpos, a->primrot, a->primscale, ws,
                           L, st);
         if (rc != MVP_OK) return rc;
     }
@@ -3094,6 +3157,7 @@ static int forward_impl(const mvp_forward_args *a, const int32_t *vset, int nset
     p.pview = pview;
     p.vset = vset; p.nsets = nsets;
     p.raycam = camera ? reinterpret_cast<const float4 *>(ws + L.raycam) : nullptr;
+    p.pix = pix;
     p.order = a->order; p.rankof = a->order ? reinterpret_cast<const int *>(ws + L.rankof) : nullptr;
     p.rgb_nchw = a->rayrgb_nchw; p.alpha_nchw = a->rayalpha_nchw;
 #if MVP_LIST_REUSE
@@ -3140,32 +3204,34 @@ static int forward_impl(const mvp_forward_args *a, const int32_t *vset, int nset
     const int cubic = (a->shape.TD == a->shape.TH && a->shape.TH == a->shape.TW) ? a->shape.TD : 0;
     int heavy = 0;
     if (int eh = heavy_grid(&heavy)) return eh;
-#define MVP_LAUNCH_FWD(TT, WW_, VV, SS)                                                                      \
+#define MVP_LAUNCH_FWD(TT, WW_, VV, SS, PP)                                                                  \
     do {                                                                                                     \
         if (a->raysat) {                                                                                     \
-            MVP_CARVE(MVP_FWD_CARVEOUT, render_forward_kernel<TT, true, kFastCapF, WW_, VV, SS>);            \
-            MVP_LAUNCH_FAST(render_forward_kernel<TT, true, kFastCapF, WW_, VV, SS>);                        \
-            MVP_LAUNCH_HEAVY(render_forward_kernel<TT, true, kMaxHit, WW_, VV, SS>);                         \
+            MVP_CARVE(MVP_FWD_CARVEOUT, render_forward_kernel<TT, true, kFastCapF, WW_, VV, SS, PP>);        \
+            MVP_LAUNCH_FAST(render_forward_kernel<TT, true, kFastCapF, WW_, VV, SS, PP>);                    \
+            MVP_LAUNCH_HEAVY(render_forward_kernel<TT, true, kMaxHit, WW_, VV, SS, PP>);                     \
         } else {                                                                                             \
-            MVP_CARVE(MVP_FWD_CARVEOUT, render_forward_kernel<TT, false, kFastCapF, WW_, VV, SS>);           \
-            MVP_LAUNCH_FAST(render_forward_kernel<TT, false, kFastCapF, WW_, VV, SS>);                       \
-            MVP_LAUNCH_HEAVY(render_forward_kernel<TT, false, kMaxHit, WW_, VV, SS>);                        \
+            MVP_CARVE(MVP_FWD_CARVEOUT, render_forward_kernel<TT, false, kFastCapF, WW_, VV, SS, PP>);       \
+            MVP_LAUNCH_FAST(render_forward_kernel<TT, false, kFastCapF, WW_, VV, SS, PP>);                   \
+            MVP_LAUNCH_HEAVY(render_forward_kernel<TT, false, kMaxHit, WW_, VV, SS, PP>);                    \
         }                                                                                                    \
     } while (0)
-#define MVP_LAUNCH_FWD_T(VV, SS)                                                                             \
+#define MVP_LAUNCH_FWD_T(VV, SS, PP)                                                                         \
     do {                                                                                                     \
-        if (a->algo == 1) MVP_LAUNCH_FWD(0, true, VV, SS);                                                   \
-        else if (cubic == 8) MVP_LAUNCH_FWD(8, false, VV, SS);                                               \
-        else if (cubic == 16) MVP_LAUNCH_FWD(16, false, VV, SS);                                             \
-        else MVP_LAUNCH_FWD(0, false, VV, SS);                                                               \
+        if (a->algo == 1) MVP_LAUNCH_FWD(0, true, VV, SS, PP);                                               \
+        else if (cubic == 8) MVP_LAUNCH_FWD(8, false, VV, SS, PP);                                           \
+        else if (cubic == 16) MVP_LAUNCH_FWD(16, false, VV, SS, PP);                                         \
+        else MVP_LAUNCH_FWD(0, false, VV, SS, PP);                                                           \
     } while (0)
-    if (vset) {
-        if (bf16) MVP_LAUNCH_FWD_T(Bf16x4, true);
-        else MVP_LAUNCH_FWD_T(float4, true);
-    } else {
-        if (bf16) MVP_LAUNCH_FWD_T(Bf16x4, false);
-        else MVP_LAUNCH_FWD_T(float4, false);
-    }
+#define MVP_LAUNCH_FWD_V(SS, PP)                                                                             \
+    do {                                                                                                     \
+        if (bf16) MVP_LAUNCH_FWD_T(Bf16x4, SS, PP);                                                          \
+        else MVP_LAUNCH_FWD_T(float4, SS, PP);                                                               \
+    } while (0)
+    if (pix) MVP_LAUNCH_FWD_V(true, true);         // with or without a map (prim_set)
+    else if (vset) MVP_LAUNCH_FWD_V(true, false);
+    else MVP_LAUNCH_FWD_V(false, false);
+#undef MVP_LAUNCH_FWD_V
 #undef MVP_LAUNCH_FWD_T
 #undef MVP_LAUNCH_FWD
     cudaError_t e = cudaGetLastError();
@@ -3175,23 +3241,25 @@ static int forward_impl(const mvp_forward_args *a, const int32_t *vset, int nset
 int mvp_raymarch_forward(const mvp_forward_args *a, void *stream) {
     if (!a) return MVP_ERR_NULL;
     if (a->struct_size != sizeof(mvp_forward_args)) return MVP_ERR_STRUCT;
-    return forward_impl(a, nullptr, 0, stream);
+    return forward_impl(a, nullptr, 0, nullptr, stream);
 }
 
 int mvp_raymarch_forward_sets(const mvp_forward_args *a, const int32_t *view_set, int32_t nsets, void *stream) {
     if (!a) return MVP_ERR_NULL;
     if (a->struct_size != sizeof(mvp_forward_args)) return MVP_ERR_STRUCT;
     const int rc = check_view_sets(a->shape, a->flags, view_set, nsets);
-    return rc != MVP_OK ? rc : forward_impl(a, view_set, nsets, stream);
+    return rc != MVP_OK ? rc : forward_impl(a, view_set, nsets, nullptr, stream);
 }
 
 // mvp_raymarch_backward, and with rays = true mvp_raymarch_backward_rays (grad_raypos / grad_raydir / grad_tminmax checked by the caller
-// for NULL; every other check is made here, before any device work); vset != NULL: the sets forms (map checked by the caller)
+// for NULL; every other check is made here, before any device work); vset != NULL: the sets forms (map checked by the caller);
+// pix != NULL: the pixels form
 static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_raypos, float *grad_raydir, float *grad_tminmax,
-                         const int32_t *vset, int nsets, void *stream) {
+                         const int32_t *vset, int nsets, const float2 *pix, void *stream) {
     const int camrc = check_camera(a->camera);
     if (camrc < 0) return camrc;
     const mvp_camera *const camera = camrc ? &a->camera : nullptr;
+    if (pix && !camera) return MVP_ERR_NULL;
     // the gradient set: MVP_FLAG_RAY_GRADS_ONLY needs the ray outputs (without them nothing would be computed)
     const bool gt = wants_tplate_grad(a->flags), gp = wants_transform_grad(a->flags);
     if (!gp && !rays) return MVP_ERR_NULL;
@@ -3221,13 +3289,13 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
         misaligned(a->primrot, 4) || misaligned(a->primscale, 4) || misaligned(a->raysat, 4) || misaligned(grad_primpos, 4) ||
         misaligned(grad_primrot, 4) || misaligned(grad_primscale, 4) || misaligned(a->warp, 4) || misaligned(grad_warp, 4) ||
         misaligned(a->grad_rayrgb_nchw, 4) || misaligned(a->grad_rayalpha_nchw, 4) || misaligned(a->order, 4) ||
-        misaligned(grad_raypos, 4) || misaligned(grad_raydir, 4) || misaligned(grad_tminmax, 8))
+        misaligned(grad_raypos, 4) || misaligned(grad_raydir, 4) || misaligned(grad_tminmax, 8) || misaligned(pix, 8))
         return MVP_ERR_ALIGN;
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)a->workspace;
     const int pview = (a->flags & MVP_FLAG_SHARED_PRIMS) ? 0 : 1;
     if (!(a->flags & MVP_FLAG_ACCEL_VALID)) {
-        rc = launch_accel(a->shape, pview, vset, nsets, a->order, a->raypos, a->raydir, camera, a->primpos, a->primrot, a->primscale, ws,
+        rc = launch_accel(a->shape, pview, vset, nsets, a->order, a->raypos, a->raydir, camera, pix, a->primpos, a->primrot, a->primscale, ws,
                           L, st);
         if (rc != MVP_OK) return rc;
     }
@@ -3247,6 +3315,7 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
     p.pview = pview;
     p.vset = vset; p.nsets = nsets;
     p.raycam = camera ? reinterpret_cast<const float4 *>(ws + L.raycam) : nullptr;
+    p.pix = pix;
     p.raypos = a->raypos; p.raydir = a->raydir; p.tminmax = a->tminmax; p.tplate = a->tplate;
     p.use_order = a->shape.N <= MVP_CTA_ORDER_MAXVIEWS;
     p.order = a->order; p.rankof = a->order ? reinterpret_cast<const int *>(ws + L.rankof) : nullptr;
@@ -3268,47 +3337,48 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
     const int cubic = (a->shape.TD == a->shape.TH && a->shape.TH == a->shape.TW) ? a->shape.TD : 0;
     int heavy = 0;
     if (int eh = heavy_grid(&heavy)) return eh;
-#define MVP_LAUNCH_BWD(TT, WW_, VV, SS)                                                                      \
+#define MVP_LAUNCH_BWD(TT, WW_, VV, SS, PP)                                                                  \
     do {                                                                                                     \
         if (rays) {                                                                                          \
-            MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV, true, kGradAll, SS>); \
-            MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV, true, kGradAll, SS>);             \
-            MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV, true, kGradAll, SS>);              \
+            MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV, true, kGradAll, SS, PP>); \
+            MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV, true, kGradAll, SS, PP>);         \
+            MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV, true, kGradAll, SS, PP>);          \
         } else {                                                                                             \
-            MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV, false, kGradAll, SS>);\
-            MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV, false, kGradAll, SS>);            \
-            MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV, false, kGradAll, SS>);             \
+            MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV, false, kGradAll, SS, PP>); \
+            MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV, false, kGradAll, SS, PP>);        \
+            MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV, false, kGradAll, SS, PP>);         \
         }                                                                                                    \
     } while (0)
     // the reduced gradient sets (float4 and Bf16x4 only: without a template gradient Bf16x4G32 is Bf16x4)
-#define MVP_LAUNCH_BWD_SET(TT, WW_, VV, RG, SET, SS)                                                         \
+#define MVP_LAUNCH_BWD_SET(TT, WW_, VV, RG, SET, SS, PP)                                                     \
     do {                                                                                                     \
-        MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV, RG, SET, SS>);            \
-        MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV, RG, SET, SS>);                        \
-        MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV, RG, SET, SS>);                         \
+        MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, WW_, VV, RG, SET, SS, PP>);        \
+        MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, WW_, VV, RG, SET, SS, PP>);                    \
+        MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, WW_, VV, RG, SET, SS, PP>);                     \
     } while (0)
-#define MVP_LAUNCH_BWD_ANY(TT, WW_, VV, SS)                                                                  \
+#define MVP_LAUNCH_BWD_ANY(TT, WW_, VV, SS, PP)                                                              \
     do {                                                                                                     \
-        if (set == kGradRaysOnly) MVP_LAUNCH_BWD_SET(TT, WW_, VV, true, kGradRaysOnly, SS);                  \
-        else if (set == kGradNoPayload && rays) MVP_LAUNCH_BWD_SET(TT, WW_, VV, true, kGradNoPayload, SS);   \
-        else if (set == kGradNoPayload) MVP_LAUNCH_BWD_SET(TT, WW_, VV, false, kGradNoPayload, SS);          \
-        else MVP_LAUNCH_BWD(TT, WW_, VV, SS);                                                                \
+        if (set == kGradRaysOnly) MVP_LAUNCH_BWD_SET(TT, WW_, VV, true, kGradRaysOnly, SS, PP);              \
+        else if (set == kGradNoPayload && rays) MVP_LAUNCH_BWD_SET(TT, WW_, VV, true, kGradNoPayload, SS, PP); \
+        else if (set == kGradNoPayload) MVP_LAUNCH_BWD_SET(TT, WW_, VV, false, kGradNoPayload, SS, PP);      \
+        else MVP_LAUNCH_BWD(TT, WW_, VV, SS, PP);                                                            \
     } while (0)
-#define MVP_LAUNCH_BWD_T(LAUNCH, VV, SS)                                                         \
-    do {                                                                                         \
-        if (a->algo == 1) LAUNCH(0, true, VV, SS);                                               \
-        else if (cubic == 8) LAUNCH(8, false, VV, SS);                                           \
-        else if (cubic == 16) LAUNCH(16, false, VV, SS);                                         \
-        else LAUNCH(0, false, VV, SS);                                                           \
-    } while (0)
-#define MVP_LAUNCH_BWD_V(SS)                                                                                 \
+#define MVP_LAUNCH_BWD_T(LAUNCH, VV, SS, PP)                                                                 \
     do {                                                                                                     \
-        if (bf16 && gwords == Payload<Bf16x4G32>::kWords && set == kGradAll) MVP_LAUNCH_BWD_T(MVP_LAUNCH_BWD, Bf16x4G32, SS); \
-        else if (bf16) MVP_LAUNCH_BWD_T(MVP_LAUNCH_BWD_ANY, Bf16x4, SS);                                     \
-        else MVP_LAUNCH_BWD_T(MVP_LAUNCH_BWD_ANY, float4, SS);                                               \
+        if (a->algo == 1) LAUNCH(0, true, VV, SS, PP);                                                       \
+        else if (cubic == 8) LAUNCH(8, false, VV, SS, PP);                                                   \
+        else if (cubic == 16) LAUNCH(16, false, VV, SS, PP);                                                 \
+        else LAUNCH(0, false, VV, SS, PP);                                                                   \
     } while (0)
-    if (vset) MVP_LAUNCH_BWD_V(true);
-    else MVP_LAUNCH_BWD_V(false);
+#define MVP_LAUNCH_BWD_V(SS, PP)                                                                             \
+    do {                                                                                                     \
+        if (bf16 && gwords == Payload<Bf16x4G32>::kWords && set == kGradAll) MVP_LAUNCH_BWD_T(MVP_LAUNCH_BWD, Bf16x4G32, SS, PP); \
+        else if (bf16) MVP_LAUNCH_BWD_T(MVP_LAUNCH_BWD_ANY, Bf16x4, SS, PP);                                 \
+        else MVP_LAUNCH_BWD_T(MVP_LAUNCH_BWD_ANY, float4, SS, PP);                                           \
+    } while (0)
+    if (pix) MVP_LAUNCH_BWD_V(true, true);
+    else if (vset) MVP_LAUNCH_BWD_V(true, false);
+    else MVP_LAUNCH_BWD_V(false, false);
 #undef MVP_LAUNCH_BWD_V
 #undef MVP_LAUNCH_BWD_T
 #undef MVP_LAUNCH_BWD_ANY
@@ -3321,14 +3391,14 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
 int mvp_raymarch_backward(const mvp_backward_args *a, void *stream) {
     if (!a) return MVP_ERR_NULL;
     if (a->struct_size != sizeof(mvp_backward_args)) return MVP_ERR_STRUCT;
-    return backward_impl(a, false, nullptr, nullptr, nullptr, nullptr, 0, stream);
+    return backward_impl(a, false, nullptr, nullptr, nullptr, nullptr, 0, nullptr, stream);
 }
 
 int mvp_raymarch_backward_rays(const mvp_backward_args *a, float *grad_raypos, float *grad_raydir, float *grad_tminmax, void *stream) {
     if (!a) return MVP_ERR_NULL;
     if (a->struct_size != sizeof(mvp_backward_args)) return MVP_ERR_STRUCT;
     if (!grad_raypos || !grad_raydir || !grad_tminmax) return MVP_ERR_NULL;
-    return backward_impl(a, true, grad_raypos, grad_raydir, grad_tminmax, nullptr, 0, stream);
+    return backward_impl(a, true, grad_raypos, grad_raydir, grad_tminmax, nullptr, 0, nullptr, stream);
 }
 
 int mvp_raymarch_backward_sets(const mvp_backward_args *a, const int32_t *view_set, int32_t nsets, float *grad_raypos, float *grad_raydir,
@@ -3338,7 +3408,27 @@ int mvp_raymarch_backward_sets(const mvp_backward_args *a, const int32_t *view_s
     const int nrays = (grad_raypos != nullptr) + (grad_raydir != nullptr) + (grad_tminmax != nullptr);
     if (nrays != 0 && nrays != 3) return MVP_ERR_NULL;
     const int rc = check_view_sets(a->shape, a->flags, view_set, nsets);
-    return rc != MVP_OK ? rc : backward_impl(a, nrays == 3, grad_raypos, grad_raydir, grad_tminmax, view_set, nsets, stream);
+    return rc != MVP_OK ? rc : backward_impl(a, nrays == 3, grad_raypos, grad_raydir, grad_tminmax, view_set, nsets, nullptr, stream);
+}
+
+int mvp_raymarch_forward_pixels(const mvp_forward_args *a, const float *pixelcoords, const int32_t *view_set, int32_t nsets, void *stream) {
+    if (!a) return MVP_ERR_NULL;
+    if (a->struct_size != sizeof(mvp_forward_args)) return MVP_ERR_STRUCT;
+    if (!pixelcoords) return MVP_ERR_NULL;
+    const int rc = view_set ? check_view_sets(a->shape, a->flags, view_set, nsets) : MVP_OK;
+    return rc != MVP_OK ? rc : forward_impl(a, view_set, view_set ? nsets : 0, reinterpret_cast<const float2 *>(pixelcoords), stream);
+}
+
+int mvp_raymarch_backward_pixels(const mvp_backward_args *a, const float *pixelcoords, const int32_t *view_set, int32_t nsets,
+                                 float *grad_raypos, float *grad_raydir, float *grad_tminmax, void *stream) {
+    if (!a) return MVP_ERR_NULL;
+    if (a->struct_size != sizeof(mvp_backward_args)) return MVP_ERR_STRUCT;
+    if (!pixelcoords) return MVP_ERR_NULL;
+    const int nrays = (grad_raypos != nullptr) + (grad_raydir != nullptr) + (grad_tminmax != nullptr);
+    if (nrays != 0 && nrays != 3) return MVP_ERR_NULL;
+    const int rc = view_set ? check_view_sets(a->shape, a->flags, view_set, nsets) : MVP_OK;
+    return rc != MVP_OK ? rc : backward_impl(a, nrays == 3, grad_raypos, grad_raydir, grad_tminmax, view_set, view_set ? nsets : 0,
+                                             reinterpret_cast<const float2 *>(pixelcoords), stream);
 }
 
 #if defined(MVP_CPU_EMUL) && defined(MVP_EMUL_STATS)

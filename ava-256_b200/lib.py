@@ -88,7 +88,7 @@ EXPORTS = ("mvp_abi_version", "mvp_build_config", "mvp_error_string", "mvp_works
            "mvp_compute_morton",
            "mvp_expand_views", "mvp_sum_views", "mvp_assemble_payload_forward_bf16", "mvp_assemble_payload_backward_bf16",
            "mvp_sum_views_bf16", "mvp_raymarch_backward_rays", "mvp_compute_raydirs_backward", "mvp_raymarch_forward_sets",
-           "mvp_raymarch_backward_sets")
+           "mvp_raymarch_backward_sets", "mvp_raymarch_forward_pixels", "mvp_raymarch_backward_pixels", "mvp_debug_view_fallback_offset")
 
 
 def _load():
@@ -131,6 +131,10 @@ def _load():
     lib.mvp_raymarch_forward_sets.argtypes = [ctypes.POINTER(ForwardArgs), c_f, ctypes.c_int32, c_f]
     lib.mvp_raymarch_backward_sets.restype = ctypes.c_int
     lib.mvp_raymarch_backward_sets.argtypes = [ctypes.POINTER(BackwardArgs), c_f, ctypes.c_int32] + [c_f] * 4
+    lib.mvp_raymarch_forward_pixels.restype = ctypes.c_int
+    lib.mvp_raymarch_forward_pixels.argtypes = [ctypes.POINTER(ForwardArgs), c_f, c_f, ctypes.c_int32, c_f]
+    lib.mvp_raymarch_backward_pixels.restype = ctypes.c_int
+    lib.mvp_raymarch_backward_pixels.argtypes = [ctypes.POINTER(BackwardArgs), c_f, c_f, ctypes.c_int32] + [c_f] * 4
     lib.mvp_compute_raydirs_backward.restype = ctypes.c_int
     lib.mvp_compute_raydirs_backward.argtypes = [ctypes.c_int32] * 3 + [c_f] * 5 + [ctypes.c_float] + [c_f] * 8
     lib.mvp_composite_forward.restype = ctypes.c_int
@@ -153,6 +157,8 @@ def _load():
     lib.mvp_sum_views_bf16.argtypes = [c_f, c_f, ctypes.c_size_t, ctypes.c_int32, ctypes.c_int32, c_f]
     lib.mvp_debug_heavy_offset.restype = ctypes.c_size_t
     lib.mvp_debug_heavy_offset.argtypes = [ctypes.POINTER(Shape)]
+    lib.mvp_debug_view_fallback_offset.restype = ctypes.c_size_t
+    lib.mvp_debug_view_fallback_offset.argtypes = [ctypes.POINTER(Shape)]
     lib.mvp_forward_launch_count.restype = ctypes.c_int
     lib.mvp_forward_launch_count.argtypes = [ctypes.c_uint32]
     lib.mvp_backward_launch_count.restype = ctypes.c_int
@@ -216,6 +222,13 @@ def require_view_sets():
     mvp_raymarch_backward_sets), which it reports as VIEW_SETS=1 in its build configuration."""
     if "VIEW_SETS=1" not in LIB.mvp_build_config().decode().split():
         raise RuntimeError("mvpraymarch_b200: this library (%s) does not support per-view primitive sets" % _build.LIB)
+
+
+def require_camera_pixels():
+    """Raise unless the library generates the camera's rays at caller-given sample positions inside the render kernels
+    (mvp_raymarch_forward_pixels, mvp_raymarch_backward_pixels), which it reports as CAMERA_PIXELS=1 in its build configuration."""
+    if "CAMERA_PIXELS=1" not in LIB.mvp_build_config().decode().split():
+        raise RuntimeError("mvpraymarch_b200: this library (%s) does not generate camera rays at sample positions" % _build.LIB)
 
 
 def workspace_bytes(N, H, W, K, TD, TH, TW):

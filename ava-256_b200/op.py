@@ -148,10 +148,15 @@ class MVPRaymarch(Function):
             raise NotImplementedError("mvpraymarch_b200: usebvh=False passes a null BVH to the reference kernels "
                                       "(mvpraymarch.py:132-134) and is not a usable mode there either")
         camera = options.get("_camera")        # (viewpos, viewrot, focal, princpt, volradius, H, W): rays generated in the kernels
+        pixels = options.get("_pixels")        # with a camera: [N,H,W,2] sample positions of its rays, or None (the integer grid)
         if camera is not None:
             assert raypos is None and raydir is None and tminmax is None
             viewpos, viewrot, focal, princpt, volradius, camH, camW = camera
-            for name, t, tail in (("viewpos", viewpos, (3,)), ("viewrot", viewrot, (3, 3)), ("focal", focal, (2,)), ("princpt", princpt, (2,))):
+            cam_tensors = (("viewpos", viewpos, (3,)), ("viewrot", viewrot, (3, 3)), ("focal", focal, (2,)), ("princpt", princpt, (2,)))
+            if pixels is not None:
+                _lib.require_camera_pixels()
+                cam_tensors += (("pixelcoords", pixels, (int(camH), int(camW), 2)),)
+            for name, t, tail in cam_tensors:
                 _check_f32_cuda(name, t)                                  # utils.py:24-25 / utils.cpp CHECK_CUDA
                 assert t.shape == (viewpos.size(0),) + tail, "%s must be [N,%s]" % (name, ",".join(map(str, tail)))
                 assert t.device == primpos.device, "%s must be on the primitives' device" % name
@@ -262,7 +267,10 @@ class MVPRaymarch(Function):
                 a.clear_grad_primpos, a.clear_grad_primrot, a.clear_grad_primscale = _ptr(grads[0]), _ptr(grads[1]), _ptr(grads[2])
                 a.clear_grad_tplate, a.clear_grad_warp = _ptr(grads[3]), _ptr(grads[4])
             stream = torch.cuda.current_stream(dev).cuda_stream
-            if view_set is not None:
+            if pixels is not None:
+                _lib.check(_lib.LIB.mvp_raymarch_forward_pixels(ctypes.byref(a), _ptr(pixels), _ptr(view_set), NP,
+                                                                ctypes.c_void_p(stream)))
+            elif view_set is not None:
                 _lib.check(_lib.LIB.mvp_raymarch_forward_sets(ctypes.byref(a), _ptr(view_set), NP, ctypes.c_void_p(stream)))
             else:
                 _lib.check(_lib.LIB.mvp_raymarch_forward(ctypes.byref(a), ctypes.c_void_p(stream)))
@@ -353,7 +361,21 @@ def _march_backward(ctx, grad_rayrgba, grad_rayalpha, want_rays):
             _lib.require_ray_grads()
             # written for every ray by the library: no zero-fill
             rays = (torch.empty((N, H, W, 3), device=dev), torch.empty((N, H, W, 3), device=dev), torch.empty((N, H, W, 2), device=dev))
-        if ctx.view_set is not None:
+        pixels = options.get("_pixels")
+        if pixels is not None and want_rays:
+            # The ray-gradient backward of a pixels forward marches the rays mvp_compute_raydirs makes from the same pixelcoords:
+            # bit for bit the rays the forward generated, so its acceleration structure and saved tile lists hold for them.  The
+            # camera's adjoint (MVPRaymarchCameraGrad) then runs mvp_compute_raydirs_backward at the same pixelcoords.
+            from .raydirs import compute_raydirs
+            viewpos, viewrot, focal, princpt, volradius = ctx.camera[:5]
+            raypos, raydir, tminmax = compute_raydirs(viewpos, viewrot, focal, princpt, pixels, volradius)
+            a.raypos, a.raydir, a.tminmax = _ptr(raypos), _ptr(raydir), _ptr(tminmax)
+            a.camera = _lib.Camera()
+            pixels = None
+        if pixels is not None:
+            _lib.check(_lib.LIB.mvp_raymarch_backward_pixels(ctypes.byref(a), _ptr(pixels), _ptr(ctx.view_set), primpos.size(0),
+                                                             *(_ptr(t) for t in (rays or (None,) * 3)), stream))
+        elif ctx.view_set is not None:
             _lib.check(_lib.LIB.mvp_raymarch_backward_sets(ctypes.byref(a), _ptr(ctx.view_set), primpos.size(0),
                                                            *(_ptr(t) for t in (rays or (None,) * 3)), stream))
         elif want_rays:
@@ -399,7 +421,7 @@ class MVPRaymarchCameraGrad(Function):
         viewpos, viewrot, focal, princpt = ctx.saved_tensors[11:15]
         volradius = ctx.camera[4]
         from .raydirs import raydirs_backward
-        cam = raydirs_backward(viewpos, viewrot, focal, princpt, None, volradius, *rays)
+        cam = raydirs_backward(viewpos, viewrot, focal, princpt, ctx.options.get("_pixels"), volradius, *rays)
         cam = tuple(g if need else None for g, need in zip(cam, ctx.needs_input_grad[:4]))
         return cam + (None,) + prim + (None, None)
 
@@ -513,6 +535,7 @@ def mvpraymarch(
         options["_view_set"] = _VIEW_SET["map"]
     if _CAMERA.get("cam") is not None:
         options["_camera"] = _CAMERA["cam"]
+        options["_pixels"] = _CAMERA.get("pix")
     if _CAMERA.get("grad"):
         options["_ray_grads"] = True
         if options.get("_camera") is not None:
@@ -527,7 +550,8 @@ def mvpraymarch(
 
 
 _PLANES = {}
-_CAMERA = {}     # "cam": the camera of a mvpraymarch_camera call (rays generated in the kernels); "grad": camera_grad=True
+_CAMERA = {}     # "cam": the camera of a mvpraymarch_camera call (rays generated in the kernels); "pix": its pixelcoords tensor or None;
+                # "grad": camera_grad=True
 _VIEW_SET = {}   # "map": the view -> primitive set map of a mvpraymarch_sets call (or of view_set= elsewhere), or None
 
 
@@ -606,17 +630,23 @@ def mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, volradius,
     """`compute_raydirs` + `mvpraymarch` of models/autoencoder.py:240-252 as ONE call: the first six parameters are those of the
     reference's compute_raydirs (extensions/utils/utils.py:48-51), the rest those of `mvpraymarch` after its ray arguments.
 
-    With `pixelcoords` given as the `(W, H)` tuple (the integer pixel grid, utils.py:28-30) the rays never exist in memory: the
-    render kernels generate each tile's rays in their prologue from the camera (C-ABI `mvp_camera`), bit-identical to what
-    `compute_raydirs` would have written -- 32 bytes per ray that are neither written by a generation pass nor read by forward
-    and backward -- and the accel build takes the camera as it is instead of fitting one to the ray field.  With a `pixelcoords`
-    tensor (arbitrary sample positions) the two calls are made one after the other, as in the reference.
+    The rays never exist in memory: the render kernels generate each tile's rays in their prologue from the camera (C-ABI
+    `mvp_camera`), bit-identical to what `compute_raydirs` would have written -- 32 bytes per ray that are neither written by a
+    generation pass nor read by forward and backward.  `pixelcoords` is the `(W, H)` tuple (the integer pixel grid, utils.py:28-30),
+    or a float32 CUDA tensor [N,H,W,2] of sample positions on the primitives' device (e.g. the dataset's meshgrid, a crop or a
+    strided sub-grid; a tensor that is not contiguous or not 8-byte aligned is copied once), from which each lane reads its own
+    position (C-ABI `mvp_raymarch_forward_pixels`).  The accel build takes the camera as it is instead of fitting one to a ray field;
+    a tensor whose views follow an axis-aligned map px = ox + sx w, py = oy + sy h keeps the slab culling, any other field renders
+    the same image with every slab a candidate (slower).  pixelcoords gets no gradient.
     By default no gradients flow to the camera, like the reference (its compute_raydirs backward returns None for every input,
     utils.py:45-46).  With camera_grad=True, viewpos, viewrot, focal and princpt are autograd inputs and those that require grad get
     the gradient of the image with every discrete decision of the march held fixed (C-ABI mvp_raymarch_backward_rays, then the ray
-    generator's adjoint mvp_compute_raydirs_backward); pixelcoords and volradius get none.  When no camera tensor requires grad,
-    the plain backward runs.  The backward computes only what requires grad: with the template and transforms detached (a frozen
-    avatar) it computes the ray gradients alone, with no template-sized gradient buffer and no payload-gradient scatter.
+    generator's adjoint mvp_compute_raydirs_backward at the same pixelcoords); pixelcoords and volradius get none.  With a
+    pixelcoords tensor the forward generates the rays in the kernels as always, and the ray-gradient backward marches the rays
+    `compute_raydirs` makes from the same tensor (bit-identical; they exist during the backward only).  When no camera tensor
+    requires grad, the plain backward runs.  The backward computes only what requires grad: with the template and transforms
+    detached (a frozen avatar) it computes the ray gradients alone, with no template-sized gradient buffer and no payload-gradient
+    scatter.
     template_grad_dtype=torch.float32 accumulates a bfloat16 template's gradient in fp32 (see the `template_grad_dtype` context
     manager); None leaves the setting of an enclosing `template_grad_dtype` block, by default the template's own dtype.
     view_set: the views render S primitive sets [S,K,...], view n set view_set[n] (see `mvpraymarch_sets`).
@@ -633,19 +663,20 @@ def mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, volradius,
     grad = bool(camera_grad) and torch.is_grad_enabled() and any(t.requires_grad for t in (viewpos, viewrot, focal, princpt))
     if grad:
         _lib.require_ray_grads()
-    if not isinstance(pixelcoords, tuple):
-        from .raydirs import compute_raydirs
-        raypos, raydir, tminmax = compute_raydirs(viewpos, viewrot, focal, princpt, pixelcoords, volradius, differentiable=grad)
-        _CAMERA["grad"] = grad
-        try:
-            return march(raypos, raydir, stepsize, tminmax, primtransf, template, warp, **kwargs)
-        finally:
-            _CAMERA["grad"] = False
-    W, H = pixelcoords
+    if isinstance(pixelcoords, tuple):
+        W, H = pixelcoords
+        pix = None
+    else:
+        if not torch.is_tensor(pixelcoords) or pixelcoords.dim() != 4:
+            raise TypeError("pixelcoords must be the (W, H) tuple or a tensor [N,H,W,2]")
+        H, W = pixelcoords.size(1), pixelcoords.size(2)
+        pix = _aligned(pixelcoords.detach().contiguous(), 8)
     _CAMERA["cam"] = (viewpos, viewrot, focal, princpt, float(volradius), int(H), int(W))
+    _CAMERA["pix"] = pix
     _CAMERA["grad"] = grad
     try:
         return march(None, None, stepsize, None, primtransf, template, warp, **kwargs)
     finally:
         _CAMERA["cam"] = None
+        _CAMERA["pix"] = None
         _CAMERA["grad"] = False

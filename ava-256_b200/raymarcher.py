@@ -46,8 +46,9 @@ class Raymarcher(nn.Module):
     def forward_camera(self, viewpos, viewrot, focal, princpt, pixelcoords, decout, renderoptions={}, rayterm=None, camera_grad=False,
                        view_set=None):
         """`compute_raydirs(viewpos, viewrot, focal, princpt, pixelcoords, volradius)` followed by `forward(raypos, raydir, tminmax,
-        ...)` -- models/autoencoder.py:240-252 -- as one call.  With `pixelcoords = (W, H)` the rays are generated inside the render
-        kernels and never stored (`op.mvpraymarch_camera`); same return tuple as `forward`.  camera_grad=True: the camera tensors
+        ...)` -- models/autoencoder.py:240-252 -- as one call.  With `pixelcoords` as the `(W, H)` tuple or as an [N,H,W,2] tensor
+        of sample positions the rays are generated inside the render kernels and never stored (`op.mvpraymarch_camera`); same
+        return tuple as `forward`.  camera_grad=True: the camera tensors
         that require grad get gradients (pose / calibration fitting through the image loss, see `op.mvpraymarch_camera`).  view_set:
         as in `forward`."""
         kwargs = dict(rayterm=rayterm, **{k: v for k, v in renderoptions.items() if k in mvpraymarch.__code__.co_varnames})

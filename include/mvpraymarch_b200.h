@@ -245,6 +245,25 @@ int mvp_raymarch_forward_sets(const mvp_forward_args *args, const int32_t *view_
 int mvp_raymarch_backward_sets(const mvp_backward_args *args, const int32_t *view_set, int32_t nsets,
                                float *grad_raypos, float *grad_raydir, float *grad_tminmax, void *stream);
 
+/* The camera form (args->camera, required: MVP_ERR_NULL without it) at arbitrary sample positions: ray (n, h, w) is the camera's ray
+ * through pixelcoords[n,h,w] (device fp32 [N,H,W,2], 8-byte aligned), the ray mvp_compute_raydirs makes from the same pixelcoords,
+ * bit for bit; no ray tensor is read or written.  The acceleration structure takes a per-view axis-aligned affine map
+ * px = ox + sx w, py = oy + sy h from three corners of the view's coordinates and verifies every coordinate against it (to 0.05 of
+ * a grid step): the integer grid, crops, strides and pixel-centre offsets keep their slab rectangles; a view that fails the check
+ * renders the same image with every slab a candidate for every tile (slower, like a ray field whose camera fit fails).
+ * view_set NULL: per-view or shared primitives as in mvp_raymarch_forward / mvp_raymarch_backward(_rays) (nsets ignored); non-NULL:
+ * the sets form, with the rules and argument errors of mvp_raymarch_forward_sets.  The backward computes the ray gradients of
+ * mvp_raymarch_backward_rays when all three ray pointers are non-NULL and none when all three are NULL (any other combination is
+ * MVP_ERR_NULL); pixelcoords gets no gradient (the camera's, via mvp_compute_raydirs_backward with the same pixelcoords).  A
+ * workspace filled by a pixels forward is valid (MVP_FLAG_ACCEL_VALID) for a pixels backward with the same pixelcoords, and for a
+ * ray-tensor backward of the rays mvp_compute_raydirs makes from them (the same rays, bit for bit).
+ * Argument errors are returned before any device work.  mvp_build_accel_camera has no pixels form.  The library supports these iff
+ * mvp_build_config() lists CAMERA_PIXELS=1. */
+int mvp_raymarch_forward_pixels(const mvp_forward_args *args, const float *pixelcoords, const int32_t *view_set, int32_t nsets,
+                                void *stream);
+int mvp_raymarch_backward_pixels(const mvp_backward_args *args, const float *pixelcoords, const int32_t *view_set, int32_t nsets,
+                                 float *grad_raypos, float *grad_raydir, float *grad_tminmax, void *stream);
+
 /* Pinhole ray generation + unit-cube clip (reference: extensions/utils/utils_kernel.cu:12-52).
  * viewpos [N,3], viewrot [N,3,3], focal [N,2], princpt [N,2], pixelcoords [N,H,W,2] or NULL (integer grid);
  * outputs raypos, raydir [N,H,W,3], tminmax [N,H,W,2]. */
@@ -322,8 +341,14 @@ size_t mvp_debug_tileclk_offset(const mvp_shape *shape);
  * tiles whose slab list did not fit the fast render kernel's list and that the 512-entry kernel rendered.  Every forward and
  * backward call resets it first, so the 4 bytes read after a call are that call's count; 0 for an invalid shape. */
 size_t mvp_debug_heavy_offset(const mvp_shape *shape);
+/* Test / diagnostics helper (host only, no device work): byte offset in the workspace of the int32 [N] per-view flags of the last
+ * acceleration build: non-zero where the view's camera could not be used to cull slabs (a failed camera fit, a degenerate camera,
+ * pixelcoords off an axis-aligned map), so that every slab was a candidate on it; 0 for an invalid shape. */
+size_t mvp_debug_view_fallback_offset(const mvp_shape *shape);
 
-/* Number of kernels the last forward / backward call of this shape launches (for bench.py's gpu_launches). */
+/* Number of kernels the last forward / backward call of this shape launches (for bench.py's gpu_launches).  A pixels call
+ * (mvp_raymarch_forward_pixels / mvp_raymarch_backward_pixels) without MVP_FLAG_ACCEL_VALID launches one more: the check of its
+ * coordinates against an affine map. */
 int mvp_forward_launch_count(uint32_t flags);
 int mvp_backward_launch_count(uint32_t flags);
 
