@@ -1177,6 +1177,10 @@ struct Params {
     int nsets;
     // pixels calls (kPix kernels only): [N,H,W,2] sample positions of the camera's rays, see fetch_ray
     const float2 *pix;
+    // deterministic backward (kDet kernels only): the int64 fixed-point sums of the four primitive gradients (indexed by kDetTplate ..
+    // kDetScale, laid out like the fp32 gradients: four entries per voxel) and their per-tensor max |value|, see det_reduce
+    long long *det_acc[4];
+    unsigned *det_max;
 };
 
 // Index of view n's primitive set: n (per-view tensors), 0 (MVP_FLAG_SHARED_PRIMS) or, in the kSets kernels, its checked map entry.
@@ -1213,8 +1217,9 @@ __device__ __forceinline__ bool tile_bucket_empty(const Params &p, int n, int tx
 // steps before their own first step are idle), so any alignment reproduces the reference; equal depth is chosen over
 // "every lane starts at its own first hit" (the reference's lock-step loop) and over a plane fitted to the first-hit
 // depths because neighbouring slabs sit at randomly different depths while the sweep planes stay coherent.
-// Returns false when the list would exceed CAP (< 512): the caller hands the tile to the 512-entry kernel.
-template <int CAP, bool kPrefetch, bool kSets, bool kPix = false>
+// Returns false when the list would exceed CAP (< 512): the caller hands the tile to the 512-entry kernel.  kOptMap: a kSets kernel
+// that also serves calls without a view-set map (prim_set).
+template <int CAP, bool kPrefetch, bool kSets, bool kPix = false, bool kOptMap = kPix>
 __device__ __forceinline__ bool build_tile_list(const Params &p, float rdt, int n, int tx, int ty, int lane, TileCtx &c,
                                                 int *s_k, int *s_iv, RowEntry *s_stage, unsigned long long *s_bar, float &t,
                                                 float &x, float &y, float &z, float &r1e, int &j0) {
@@ -1236,7 +1241,7 @@ __device__ __forceinline__ bool build_tile_list(const Params &p, float rdt, int 
     march_margins(c.ray, rdt, epos, eps0);
 #endif
 
-    const float4 *packn = p.pack + (size_t)prim_set<kSets, kPix>(p, n) * p.K * 4;
+    const float4 *packn = p.pack + (size_t)prim_set<kSets, kOptMap>(p, n) * p.K * 4;
     const int cnt = p.rowcnt[(size_t)n * p.R + ty];
     const bool overflow = cnt > p.rowcap;
 #if MVP_XBUCKETS
@@ -1286,7 +1291,7 @@ __device__ __forceinline__ bool build_tile_list(const Params &p, float rdt, int 
                 k = e.k; xr = e.xr;
                 cand = true;
             } else {
-                k = slab_at_rank(p.order ? p.order + (size_t)prim_set<kSets, kPix>(p, n) * p.K : nullptr, p.K, kstart, idx);
+                k = slab_at_rank(p.order ? p.order + (size_t)prim_set<kSets, kOptMap>(p, n) * p.K : nullptr, p.K, kstart, idx);
                 xr = __ldg(rxn + k);
                 unsigned yr = __ldg(ryn + k);
                 int y0 = (int)(yr & 0xffffu), y1 = (int)(yr >> 16);
@@ -1354,7 +1359,7 @@ __device__ __forceinline__ bool build_tile_list(const Params &p, float rdt, int 
     // TMA bulk prefetch (cp.async.bulk.prefetch.L2): pull the payload slabs this tile is about to sample into L2 while
     // the lattice set-up runs; one lane per slab, fire and forget.
     if (kPrefetch && p.slab_bytes >= 16) {
-        const char *tp = reinterpret_cast<const char *>(p.tplate) + (size_t)prim_set<kSets, kPix>(p, n) * p.K * p.slab_bytes;
+        const char *tp = reinterpret_cast<const char *>(p.tplate) + (size_t)prim_set<kSets, kOptMap>(p, n) * p.K * p.slab_bytes;
         for (int i = lane; i < nl; i += 32) {
             const char *a = tp + (size_t)s_k[i] * p.slab_bytes;
             asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(a), "r"(p.slab_bytes) : "memory");
@@ -1524,6 +1529,100 @@ template <> struct Payload<Bf16x4G32> {
     static __device__ __forceinline__ float4 load(const Bf16x4G32 *v) { return Payload<Bf16x4>::load(reinterpret_cast<const Bf16x4 *>(v)); }
     static __device__ __forceinline__ void red(float *g, size_t i, float a, float b, float c, float d) { red_add_v4(g + i * 4, a, b, c, d); }
 };
+
+// ---- deterministic backward (MVP_FLAG_DETERMINISTIC): the primitive gradients summed in 64-bit two's-complement fixed point ----
+// The backward runs twice with every global reduction of a primitive gradient replaced.  kDetMeasure: each value goes into a
+// per-tensor max of |x| (the bit patterns of non-negative floats order like the floats, so atomicMax on them is order-free); a
+// non-finite value instead marks its entry with kDetPoison.  kDetAccumulate: each finite value is added as llrint(x / q) with a
+// 64-bit integer reduction, q = 2^det_quantum_exp(max) the tensor's quantum.  Integer addition is associative, so the sums do not
+// depend on the order of the reductions; det_convert_kernel then writes (float)sum * q.
+// Headroom: 2^(e+38) >= max |x|, so every term is at most 2^38 in magnitude and an entry stays below 2^62 for fewer than 2^24
+// reductions into it.  An entry poisoned by the measure pass holds 2^63 + (a sum below 2^62): its two top bits differ, and only
+// such entries convert to NaN.
+constexpr int kDetOff = 0, kDetMeasure = 1, kDetAccumulate = 2;
+constexpr int kDetTplate = 0, kDetPos = 1, kDetRot = 2, kDetScale = 3;   // index of a primitive gradient in Params::det_acc / det_max
+constexpr int kDetFracBits = 38;
+constexpr unsigned long long kDetPoison = 0x8000000000000000ull;
+
+// exponent of the quantum of a tensor whose largest finite |value| has the fp32 bit pattern mbits: (the smallest e with 2^e >= max)
+// - 38, at least -126 so that q and 1/q are normal floats (a tensor of zeros gets -126)
+__host__ __device__ inline int det_quantum_exp(unsigned mbits) {
+    const int ex = (int)(mbits >> 23) - 127;                         // max = 1.m * 2^ex (mbits < 0x7f800000: finite, non-negative)
+    const int e = (mbits & 0x7fffffu) ? ex + 1 : ex;                 // smallest power of two >= max
+    const int qe = e - kDetFracBits;
+    return qe < -126 ? -126 : qe;
+}
+__device__ __forceinline__ float det_pow2(int e) { return __uint_as_float((unsigned)(127 + e) << 23); }   // -126 <= e <= 127
+
+__device__ __forceinline__ bool det_finite(float x) { return (__float_as_uint(x) & 0x7fffffffu) < 0x7f800000u; }
+
+// The integer reductions and conversions of the fixed point.  The CPU emulation of the kernels (tests/emul/) has none of them: there
+// they are the same operations on host atomics (cvt.rni.s64.f32 = llrint; the values stay far inside the int64 range).
+__device__ __forceinline__ void det_red_add_u64(unsigned long long *a, long long v) {
+#ifdef MVP_CPU_EMUL
+    std::atomic_ref<unsigned long long>(*a).fetch_add((unsigned long long)v, std::memory_order_relaxed);
+#else
+    atomicAdd(a, (unsigned long long)v);
+#endif
+}
+__device__ __forceinline__ void det_red_max_u32(unsigned *a, unsigned v) {
+#ifdef MVP_CPU_EMUL
+    std::atomic_ref<unsigned> r(*a);
+    unsigned old = r.load(std::memory_order_relaxed);
+    while (old < v && !r.compare_exchange_weak(old, v, std::memory_order_relaxed)) {}
+#else
+    atomicMax(a, v);
+#endif
+}
+__device__ __forceinline__ long long det_f2ll_rn(float x) {
+#ifdef MVP_CPU_EMUL
+    return std::llrint(x);
+#else
+    return __float2ll_rn(x);
+#endif
+}
+__device__ __forceinline__ float det_ll2f_rn(long long x) {
+#ifdef MVP_CPU_EMUL
+    return (float)x;     // round to nearest: the host's default rounding mode
+#else
+    return __ll2float_rn(x);
+#endif
+}
+
+// One reduction of value x into entry i of primitive gradient t, in the pass kDet: the measure pass raises this lane's running
+// max mx (flushed once per tile, det_flush_max), the accumulate pass adds the fixed-point value.
+template <int kDet>
+__device__ __forceinline__ void det_reduce(const Params &p, int t, size_t i, float x, unsigned &mx) {
+    if (kDet == kDetMeasure) {
+        if (det_finite(x)) mx = max(mx, __float_as_uint(x) & 0x7fffffffu);
+        else reinterpret_cast<unsigned long long *>(p.det_acc[t])[i] = kDetPoison;   // the same store from every writer: order-free
+    } else if (det_finite(x)) {
+        const float s = det_pow2(-det_quantum_exp(__ldg(p.det_max + t)));           // 1/q: x * s is exact
+        det_red_add_u64(reinterpret_cast<unsigned long long *>(p.det_acc[t]) + i, det_f2ll_rn(x * s));
+    }
+}
+
+// The measure pass's per-lane maxima into the per-tensor maxima: one warp reduction and one atomic per tensor and tile.
+__device__ __forceinline__ void det_flush_max(const Params &p, int lane, const unsigned (&mx)[4]) {
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+        const unsigned m = __reduce_max_sync(0xffffffffu, mx[t]);
+        if (lane == 0 && m) det_red_max_u32(p.det_max + t, m);
+    }
+}
+
+// (float)sum * q of every entry of one primitive gradient, NaN where the measure pass saw a non-finite value; written as fp32 or,
+// with bf16, rounded once more to bfloat16 (nearest even).  One thread per entry.
+__global__ void __launch_bounds__(256) det_convert_kernel(size_t n, const long long *__restrict__ acc, const unsigned *__restrict__ det_max,
+                                                          int t, float *__restrict__ out, int bf16) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const long long s = acc[i];
+    const float q = det_pow2(det_quantum_exp(det_max[t]));
+    const float v = ((s >> 62) != (s >> 63)) ? __uint_as_float(0x7fc00000u) : det_ll2f_rn(s) * q;
+    if (bf16) reinterpret_cast<unsigned short *>(out)[i] = (unsigned short)(cvt_bf16x2(0.f, v) & 0xffffu);
+    else out[i] = v;
+}
 
 // primsampler.h:44-66 + utils.h:408-502.  T > 0: cubic slab with compile-time strides; T == 0: runtime dims.
 // Only called for valid samples (|y| < 1), for which (a) the reference's +-100 clamp is a no-op and (b) the only
@@ -2135,9 +2234,12 @@ constexpr int kGradAll = 0;         // transforms, template (+ warp field)
 constexpr int kGradNoPayload = 1;   // transforms only (MVP_FLAG_NO_TPLATE_GRAD): no payload-gradient scatter
 constexpr int kGradRaysOnly = 2;    // ray gradients only (MVP_FLAG_RAY_GRADS_ONLY; kRayGrad kernels): no transform sums either
 
-template <int T, int CAP, bool kWarp, typename V, bool kRayGrad, int kSet, bool kSets, bool kPix>
+template <int T, int CAP, bool kWarp, typename V, bool kRayGrad, int kSet, bool kSets, bool kPix, int kDet>
 __device__ __forceinline__ bool backward_tile(const Params &p, const int n, const int tx, const int ty, const int lane, BwdWarpSmem<CAP> *const S) {
     static_assert(kSet != kGradRaysOnly || kRayGrad, "a rays-only backward computes the ray gradients");
+    static_assert(kDet == kDetOff || (!kWarp && !kRayGrad && kSets && kSet != kGradRaysOnly), "deterministic: algo 0, primitive gradients");
+    constexpr bool kOptMap = kPix || kDet != kDetOff;   // the deterministic kernels serve calls with and without a view-set map
+    unsigned dmx[4] = {0u, 0u, 0u, 0u};                 // kDetMeasure: this lane's max |value| per primitive gradient
     int *const sk = S->k, *const siv = S->iv;
     RowEntry *const sstage = S->stage;
     unsigned long long *const sbar = S->bar;
@@ -2155,7 +2257,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
     have = load_saved_tile_list<CAP, kPix>(p, rdt, n, tx, ty, lane, c, sk, siv, xb, yb, zb, j0);
     if (have == 2) return false;
 #endif
-    if (have == 0 && !build_tile_list<CAP, false, kSets, kPix>(p, rdt, n, tx, ty, lane, c, sk, siv, sstage, sbar, t0, xb, yb, zb, r1e, j0)) return false;
+    if (have == 0 && !build_tile_list<CAP, false, kSets, kPix, kOptMap>(p, rdt, n, tx, ty, lane, c, sk, siv, sstage, sbar, t0, xb, yb, zb, r1e, j0)) return false;
     const int nl = c.nl;
     if (nl == 0) {
         if (kRayGrad) store_ray_grads(p, n, tx, ty, lane, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f);
@@ -2204,11 +2306,11 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
         return true;
     }
 
-    const float4 *packn = p.pack + (size_t)prim_set<kSets, kPix>(p, n) * p.K * 4;
+    const float4 *packn = p.pack + (size_t)prim_set<kSets, kOptMap>(p, n) * p.K * 4;
     const size_t slabsz = (size_t)p.TD * p.TH * p.TW;   // (a compile-time T^3 here makes the compiler keep slab addresses in registers: 64 B of spills)
     // bases of the primitive tensors are re-derived from the parameter block where they are used (cheap constant-bank
     // arithmetic) instead of living in a dozen registers for the whole tile
-    const size_t pvK = (size_t)prim_set<kSets, kPix>(p, n) * p.K;
+    const size_t pvK = (size_t)prim_set<kSets, kOptMap>(p, n) * p.K;
     const int td = T > 0 ? T : p.TD, th = T > 0 ? T : p.TH, tw = T > 0 ? T : p.TW;
     const float gmx = (float)(tw - 1) * 0.5f, gmy = (float)(th - 1) * 0.5f, gmz = (float)(td - 1) * 0.5f;
     const int sx = tw > 1 ? 1 : 0, sy = th > 1 ? tw : 0, sz = td > 1 ? th * tw : 0;
@@ -2277,7 +2379,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                 word &= word - 1;
                 const int slot = w * 32 + bit;
                 const int k = sk[slot];
-                const int rank = rank_of_slab(p.rankof ? p.rankof + (size_t)prim_set<kSets, kPix>(p, n) * p.K : nullptr, p.K, kstart, k);
+                const int rank = rank_of_slab(p.rankof ? p.rankof + (size_t)prim_set<kSets, kOptMap>(p, n) * p.K : nullptr, p.K, kstart, k);
 #if MVP_BWD_SMEMREC
                 __syncwarp();                                  // the previous slab's last readers of the record are done
                 if (lane < 4) S->rec[lane] = __ldg(packn + (size_t)k * 4 + lane);
@@ -2336,7 +2438,7 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                 if (maxlen <= 0) continue;
                 const V *slab = reinterpret_cast<const V *>(p.tplate) + (pvK + k) * slabsz;
                 // as 4-byte words, see Payload (kGradAll only: the other sets do not touch p.g_tplate)
-                float *gslab = kSet == kGradAll ? p.g_tplate + (pvK + k) * slabsz * Payload<V>::kWords : nullptr;
+                float *gslab = kSet == kGradAll && kDet == kDetOff ? p.g_tplate + (pvK + k) * slabsz * Payload<V>::kWords : nullptr;
                 // transform-gradient accumulators of THIS lane for this slab: Gx[i][j] = sum xm_i * dL/dy_j and
                 // Gy[j] = sum dL/dy_j; grad_rot/scale/pos are linear in them (derived once per slab, before the reduction)
 #if MVP_BWD_LANESMEM
@@ -2525,8 +2627,16 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                                 nx = __shfl_sync(0xffffffffu, nx, src);
                             }
                             if (lead) {
-                                Payload<V>::red(gc, (size_t)o, ua, ub, uc, ud);
-                                Payload<V>::red(gc, (size_t)(o + sx), ea, eb, ec, ed);
+                                if constexpr (kDet == kDetOff) {
+                                    Payload<V>::red(gc, (size_t)o, ua, ub, uc, ud);
+                                    Payload<V>::red(gc, (size_t)(o + sx), ea, eb, ec, ed);
+                                } else {
+                                    const size_t e0 = ((pvK + k) * slabsz + (size_t)(base + o)) * 4, e1 = e0 + (size_t)sx * 4;
+                                    det_reduce<kDet>(p, kDetTplate, e0, ua, dmx[0]); det_reduce<kDet>(p, kDetTplate, e0 + 1, ub, dmx[0]);
+                                    det_reduce<kDet>(p, kDetTplate, e0 + 2, uc, dmx[0]); det_reduce<kDet>(p, kDetTplate, e0 + 3, ud, dmx[0]);
+                                    det_reduce<kDet>(p, kDetTplate, e1, ea, dmx[0]); det_reduce<kDet>(p, kDetTplate, e1 + 1, eb, dmx[0]);
+                                    det_reduce<kDet>(p, kDetTplate, e1 + 2, ec, dmx[0]); det_reduce<kDet>(p, kDetTplate, e1 + 3, ed, dmx[0]);
+                                }
                             }
                         }
 #if defined(MVP_CPU_EMUL) && defined(MVP_EMUL_STATS)
@@ -2565,8 +2675,8 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                         } else {
                         // ---- algo 1 (PrimSamplerTW<true>): payload sampled at the warp-field-displaced position ----
                         const size_t wsl = (size_t)p.WD * p.WH * p.WW * 3;
-                        const float *wk = p.warp + ((size_t)prim_set<kSets, kPix>(p, n) * p.K + k) * wsl;
-                        float *gwk = kSet == kGradAll ? p.g_warp + ((size_t)prim_set<kSets, kPix>(p, n) * p.K + k) * wsl : nullptr;
+                        const float *wk = p.warp + ((size_t)prim_set<kSets, kOptMap>(p, n) * p.K + k) * wsl;
+                        float *gwk = kSet == kGradAll ? p.g_warp + ((size_t)prim_set<kSets, kOptMap>(p, n) * p.K + k) * wsl : nullptr;
                         const float e1 = p.fadeexp - 1.f;
                         const float pw0 = __powf(fabsf(y0), e1), pw1 = __powf(fabsf(y1), e1), pw2 = __powf(fabsf(y2), e1);
                         const float fade = __expf(-p.fadescale * (pw0 * fabsf(y0) + pw1 * fabsf(y1) + pw2 * fabsf(y2)));
@@ -2728,13 +2838,22 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
                 g[0] += __shfl_xor_sync(0xffffffffu, g[0], 1);
                 const int vi = lane >> 1;
                 if (!(lane & 1) && vi < 15) {
-                    float *dst = vi < 3 ? (p.g_primscale + (pvK + k) * 3 + vi)
-                                        : (vi < 12 ? (p.g_primrot + (pvK + k) * 9 + (vi - 3)) : (p.g_primpos + (pvK + k) * 3 + (vi - 12)));
-                    atomicAdd(dst, g[0]);
+                    if constexpr (kDet == kDetOff) {
+                        float *dst = vi < 3 ? (p.g_primscale + (pvK + k) * 3 + vi)
+                                            : (vi < 12 ? (p.g_primrot + (pvK + k) * 9 + (vi - 3)) : (p.g_primpos + (pvK + k) * 3 + (vi - 12)));
+                        atomicAdd(dst, g[0]);
+                    } else if (vi < 3) {
+                        det_reduce<kDet>(p, kDetScale, (pvK + k) * 3 + vi, g[0], dmx[3]);
+                    } else if (vi < 12) {
+                        det_reduce<kDet>(p, kDetRot, (pvK + k) * 9 + (vi - 3), g[0], dmx[2]);
+                    } else {
+                        det_reduce<kDet>(p, kDetPos, (pvK + k) * 3 + (vi - 12), g[0], dmx[1]);
+                    }
                 }
             }   // while (word)
         }       // for (w)
     }           // for (cs)
+    if (kDet == kDetMeasure) det_flush_max(p, lane, dmx);
     if (kRayGrad) {
         const float *ra = sra + lane;
         store_ray_grads(p, n, tx, ty, lane, ra[0 * 32], ra[1 * 32], ra[2 * 32], ra[3 * 32], ra[4 * 32], ra[5 * 32],
@@ -2746,7 +2865,10 @@ __device__ __forceinline__ bool backward_tile(const Params &p, const int n, cons
 // kRayGrad: also write the per-ray gradients p.g_raypos / g_raydir / g_tminmax (mvp_raymarch_backward_rays); false compiles to
 // the plain backward.  kSet: the gradient set (kGradAll, kGradNoPayload, kGradRaysOnly); the default is the full backward.  kSets: a
 // sets call (mvp_raymarch_backward_sets), as in render_forward_kernel; kPix: a pixels call (mvp_raymarch_backward_pixels), as there.
-template <int T, int CAP, bool kWarp, typename V, bool kRayGrad = false, int kSet = kGradAll, bool kSets = false, bool kPix = false>
+// kDet: a pass of the deterministic backward (mvp_raymarch_backward_deterministic, kSets kernels with or without a map): kDetMeasure or
+// kDetAccumulate, see det_reduce.
+template <int T, int CAP, bool kWarp, typename V, bool kRayGrad = false, int kSet = kGradAll, bool kSets = false, bool kPix = false,
+          int kDet = kDetOff>
 __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_BWD_MINB * 4) / kWarps : 12 / kWarps) render_backward_kernel(const Params p) {
     __shared__ typename BwdSmemOf<CAP, kRayGrad>::type s_w[kWarps];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -2756,7 +2878,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         for (int i = blockIdx.x * kWarps + warp; i < cnt; i += gridDim.x * kWarps) {
             const int id = p.heavylist[i];
             const int tx = id % p.TXn, ty = (id / p.TXn) % p.TYn, n = id / (p.TXn * p.TYn);
-            backward_tile<T, CAP, kWarp, V, kRayGrad, kSet, kSets, kPix>(p, n, tx, ty, lane, S);
+            backward_tile<T, CAP, kWarp, V, kRayGrad, kSet, kSets, kPix, kDet>(p, n, tx, ty, lane, S);
             __syncwarp();
         }
     } else {
@@ -2769,7 +2891,7 @@ __global__ void __launch_bounds__(kWarps * 32, (CAP < kMaxHit && !kWarp) ? (MVP_
         const int tx = blockIdx.x * kBlkTX + (warp % kBlkTX), ty = blockIdx.y * kBlkTY + (warp / kBlkTX), n = blockIdx.z;
 #endif
         if (tx >= p.TXn || ty >= p.TYn) return;
-        if (!backward_tile<T, CAP, kWarp, V, kRayGrad, kSet, kSets, kPix>(p, n, tx, ty, lane, S) && lane == 0)
+        if (!backward_tile<T, CAP, kWarp, V, kRayGrad, kSet, kSets, kPix, kDet>(p, n, tx, ty, lane, S) && lane == 0)
             p.heavylist[atomicAdd(p.heavycnt, 1)] = (n * p.TYn + ty) * p.TXn + tx;
     }
 }
@@ -2996,7 +3118,7 @@ const char *mvp_build_config(void) {
     return "LIST_REUSE=" MVP_STR(MVP_LIST_REUSE)
            " LIST_MARGIN=" MVP_STR(MVP_LIST_MARGIN) " XBUCKETS=" MVP_STR(MVP_XBUCKETS) " FASTCAP=" MVP_STR(MVP_FWD_FASTCAP) "/" MVP_STR(MVP_BWD_FASTCAP) " SMEM_UNION=" MVP_STR(MVP_SMEM_UNION) " CARVEOUT=" MVP_STR(MVP_FWD_CARVEOUT) "/" MVP_STR(MVP_BWD_CARVEOUT) " FWD_RING=" MVP_STR(MVP_FWD_RING) " BWD_SMEMREC=" MVP_STR(MVP_BWD_SMEMREC) " BWD_LANESMEM=" MVP_STR(MVP_BWD_LANESMEM) " CTA_ORDER=" MVP_STR(MVP_CTA_ORDER) " CTA_ORDER_MIN=" MVP_STR(MVP_CTA_ORDER_MIN)
            " CHUNK=" MVP_STR(MVP_CHUNK) " FWD_MINB=" MVP_STR(MVP_FWD_MINB) " BWD_MINB=" MVP_STR(MVP_BWD_MINB)
-           " WARPS=" MVP_STR(MVP_WARPS) " BLK_TX=" MVP_STR(MVP_BLK_TX) " TPLATE_BF16=1 EPILOGUE_BF16=1 RAY_GRADS=1 GRAD_TPLATE_F32=1 GRAD_SELECT=1 VIEW_SETS=1 CAMERA_PIXELS=1"
+           " WARPS=" MVP_STR(MVP_WARPS) " BLK_TX=" MVP_STR(MVP_BLK_TX) " TPLATE_BF16=1 EPILOGUE_BF16=1 RAY_GRADS=1 GRAD_TPLATE_F32=1 GRAD_SELECT=1 VIEW_SETS=1 CAMERA_PIXELS=1 DETERMINISTIC=1"
 #ifdef MVP_CPU_EMUL
            " CPU_EMUL"
 #endif
@@ -3181,8 +3303,11 @@ static int forward_impl(const mvp_forward_args *a, const int32_t *vset, int nset
         // gradient buffers to clear for the coming backward: in the fast render kernel (one slice per warp), see clear_grad_slices
         const size_t nk = (size_t)(vset ? nsets : pview ? a->shape.N : 1) * a->shape.K;
         float *const bufs[kClearBufs] = {clr_primpos, clr_primrot, clr_primscale, clr_tplate, a->algo == 1 ? clr_warp : nullptr};
-        // sizes in 4-byte words: a bf16 template gradient holds two channels per word
-        const size_t floats[kClearBufs] = {nk * 3, nk * 9, nk * 3, nk * a->shape.TD * a->shape.TH * a->shape.TW * grad_tplate_words(a->flags),
+        // sizes in 4-byte words: a bf16 template gradient holds two channels per word; MVP_FLAG_DETERMINISTIC: the int64 sums of
+        // mvp_raymarch_backward_deterministic, two words per entry and four entries per voxel whatever the template's type
+        const size_t dw = (a->flags & MVP_FLAG_DETERMINISTIC) ? 2 : 1;
+        const size_t floats[kClearBufs] = {nk * 3 * dw, nk * 9 * dw, nk * 3 * dw,
+                                           nk * a->shape.TD * a->shape.TH * a->shape.TW * (dw == 2 ? 8 : grad_tplate_words(a->flags)),
                                            a->algo == 1 ? nk * a->WD * a->WH * a->WW * 3 : 0};
         for (int b = 0; b < kClearBufs; ++b) {
             if (!bufs[b]) continue;
@@ -3253,9 +3378,10 @@ int mvp_raymarch_forward_sets(const mvp_forward_args *a, const int32_t *view_set
 
 // mvp_raymarch_backward, and with rays = true mvp_raymarch_backward_rays (grad_raypos / grad_raydir / grad_tminmax checked by the caller
 // for NULL; every other check is made here, before any device work); vset != NULL: the sets forms (map checked by the caller);
-// pix != NULL: the pixels form
+// pix != NULL: the pixels form; det != NULL: mvp_raymarch_backward_deterministic (no ray gradients)
+struct DetBufs { long long *acc[4]; unsigned *max; };   // indexed by kDetTplate .. kDetScale
 static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_raypos, float *grad_raydir, float *grad_tminmax,
-                         const int32_t *vset, int nsets, const float2 *pix, void *stream) {
+                         const int32_t *vset, int nsets, const float2 *pix, void *stream, const DetBufs *det = nullptr) {
     const int camrc = check_camera(a->camera);
     if (camrc < 0) return camrc;
     const mvp_camera *const camera = camrc ? &a->camera : nullptr;
@@ -3277,6 +3403,7 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
     int rc = check_shape(a->shape);
     if (rc != MVP_OK) return rc;
     if (a->algo != 0 && a->algo != 1) return MVP_ERR_ALGO;
+    if (det && a->algo != 0) return MVP_ERR_ALGO;     // the warp field's gradient has no fixed-point form
     if (a->algo == 1 && (!a->warp || (gt && !grad_warp) || a->WD < 1 || a->WH < 1 || a->WW < 1))
         return (a->warp && (grad_warp || !gt)) ? MVP_ERR_SHAPE : MVP_ERR_NULL;
     if (!(a->stepsize > 0.f) || !(a->stepsize < 3.0e38f)) return MVP_ERR_STEPSIZE;
@@ -3284,6 +3411,12 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
     if (a->workspace_bytes < L.total || ((uintptr_t)a->workspace & 255)) return MVP_ERR_WORKSPACE;
     const bool bf16 = (a->flags & MVP_FLAG_TPLATE_BF16) != 0;
     const unsigned gwords = grad_tplate_words(a->flags);
+    if (det) {
+        if (!det->acc[kDetPos] || !det->acc[kDetRot] || !det->acc[kDetScale] || (gt && !det->acc[kDetTplate]) || !det->max) return MVP_ERR_NULL;
+        if (misaligned(det->acc[kDetPos], 8) || misaligned(det->acc[kDetRot], 8) || misaligned(det->acc[kDetScale], 8) ||
+            misaligned(gt ? det->acc[kDetTplate] : nullptr, 8) || misaligned(det->max, 4))
+            return MVP_ERR_ALIGN;
+    }
     if (misaligned(a->tplate, bf16 ? 8 : 16) || misaligned(grad_tplate, gwords * 4) || misaligned(a->grad_rayrgba, 16) || misaligned(a->rayaux, 16) ||
         misaligned(a->tminmax, 8) || misaligned(a->raypos, 4) || misaligned(a->raydir, 4) || misaligned(a->primpos, 4) ||
         misaligned(a->primrot, 4) || misaligned(a->primscale, 4) || misaligned(a->raysat, 4) || misaligned(grad_primpos, 4) ||
@@ -3299,7 +3432,18 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
                           L, st);
         if (rc != MVP_OK) return rc;
     }
-    if (a->flags & MVP_FLAG_ZERO_GRADS) {     // the requested buffers only
+    if (det) {     // the sums start at zero (the forward's clear or MVP_FLAG_ZERO_GRADS), the maxima here
+        const size_t nk = (size_t)(vset ? nsets : pview ? a->shape.N : 1) * a->shape.K;
+        cudaError_t z = cudaMemsetAsync(det->max, 0, 4 * sizeof(unsigned), st);
+        if (a->flags & MVP_FLAG_ZERO_GRADS) {
+            if (z == cudaSuccess) z = cudaMemsetAsync(det->acc[kDetPos], 0, nk * 3 * sizeof(long long), st);
+            if (z == cudaSuccess) z = cudaMemsetAsync(det->acc[kDetRot], 0, nk * 9 * sizeof(long long), st);
+            if (z == cudaSuccess) z = cudaMemsetAsync(det->acc[kDetScale], 0, nk * 3 * sizeof(long long), st);
+            if (gt && z == cudaSuccess)
+                z = cudaMemsetAsync(det->acc[kDetTplate], 0, nk * a->shape.TD * a->shape.TH * a->shape.TW * 4 * sizeof(long long), st);
+        }
+        if (z != cudaSuccess) return (int)z;
+    } else if (a->flags & MVP_FLAG_ZERO_GRADS) {     // the requested buffers only
         const size_t nk = (size_t)(vset ? nsets : pview ? a->shape.N : 1) * a->shape.K;
         cudaError_t z = cudaSuccess;
         if (gp) z = cudaMemsetAsync(grad_primpos, 0, nk * 3 * sizeof(float), st);
@@ -3337,6 +3481,59 @@ static int backward_impl(const mvp_backward_args *a, bool rays, float *grad_rayp
     const int cubic = (a->shape.TD == a->shape.TH && a->shape.TH == a->shape.TW) ? a->shape.TD : 0;
     int heavy = 0;
     if (int eh = heavy_grid(&heavy)) return eh;
+    if (det) {
+        // measure pass, accumulate pass (the heavy-tile list is refilled by its fast kernel), conversion.  Only kSets kernels: they
+        // serve calls without a map too (prim_set); the template is read as Bf16x4 whatever its gradient's type.
+        for (int t = 0; t < 4; ++t) p.det_acc[t] = det->acc[t];
+        p.det_max = det->max;
+        p.g_primpos = p.g_primrot = p.g_primscale = p.g_tplate = nullptr;
+#define MVP_LAUNCH_DET(TT, VV, SET, PP, DET)                                                                 \
+    do {                                                                                                     \
+        MVP_CARVE(MVP_BWD_CARVEOUT, render_backward_kernel<TT, kFastCapB, false, VV, false, SET, true, PP, DET>); \
+        MVP_LAUNCH_FAST(render_backward_kernel<TT, kFastCapB, false, VV, false, SET, true, PP, DET>);        \
+        MVP_LAUNCH_HEAVY(render_backward_kernel<TT, kMaxHit, false, VV, false, SET, true, PP, DET>);         \
+    } while (0)
+#define MVP_LAUNCH_DET_T(VV, SET, PP, DET)                                                                   \
+    do {                                                                                                     \
+        if (cubic == 8) MVP_LAUNCH_DET(8, VV, SET, PP, DET);                                                 \
+        else if (cubic == 16) MVP_LAUNCH_DET(16, VV, SET, PP, DET);                                          \
+        else MVP_LAUNCH_DET(0, VV, SET, PP, DET);                                                            \
+    } while (0)
+#define MVP_LAUNCH_DET_S(VV, PP, DET)                                                                        \
+    do {                                                                                                     \
+        if (set == kGradAll) MVP_LAUNCH_DET_T(VV, kGradAll, PP, DET);                                        \
+        else MVP_LAUNCH_DET_T(VV, kGradNoPayload, PP, DET);                                                  \
+    } while (0)
+#define MVP_LAUNCH_DET_V(DET)                                                                                \
+    do {                                                                                                     \
+        if (bf16 && pix) MVP_LAUNCH_DET_S(Bf16x4, true, DET);                                                \
+        else if (bf16) MVP_LAUNCH_DET_S(Bf16x4, false, DET);                                                 \
+        else if (pix) MVP_LAUNCH_DET_S(float4, true, DET);                                                   \
+        else MVP_LAUNCH_DET_S(float4, false, DET);                                                           \
+    } while (0)
+        MVP_LAUNCH_DET_V(kDetMeasure);
+        cudaError_t e0 = cudaMemsetAsync(p.heavycnt, 0, sizeof(int), st);
+        if (e0 != cudaSuccess) return (int)e0;
+        MVP_LAUNCH_DET_V(kDetAccumulate);
+#undef MVP_LAUNCH_DET_V
+#undef MVP_LAUNCH_DET_S
+#undef MVP_LAUNCH_DET_T
+#undef MVP_LAUNCH_DET
+        const size_t nk = (size_t)(vset ? nsets : pview ? a->shape.N : 1) * a->shape.K;
+        const size_t cnt[4] = {gt ? nk * a->shape.TD * a->shape.TH * a->shape.TW * 4 : 0, nk * 3, nk * 9, nk * 3};
+        float *const out[4] = {grad_tplate, grad_primpos, grad_primrot, grad_primscale};
+        for (int t = 0; t < 4; ++t) {
+            if (!cnt[t]) continue;
+            const int ob = t == kDetTplate && gwords == Payload<Bf16x4>::kWords;     // a bf16 template gradient
+#ifdef MVP_CPU_EMUL
+            MVP_LAUNCH(det_convert_kernel, (unsigned)((cnt[t] + 255) / 256), 256, 0, st, cnt[t], det->acc[t], det->max, t, out[t], ob);
+#else
+            det_convert_kernel<<<(unsigned)((cnt[t] + 255) / 256), 256, 0, st>>>(cnt[t], det->acc[t], det->max, t, out[t], ob);
+#endif
+        }
+        cudaError_t e = cudaGetLastError();
+        return e == cudaSuccess ? MVP_OK : (int)e;
+    }
 #define MVP_LAUNCH_BWD(TT, WW_, VV, SS, PP)                                                                  \
     do {                                                                                                     \
         if (rays) {                                                                                          \
@@ -3430,6 +3627,26 @@ int mvp_raymarch_backward_pixels(const mvp_backward_args *a, const float *pixelc
     return rc != MVP_OK ? rc : backward_impl(a, nrays == 3, grad_raypos, grad_raydir, grad_tminmax, view_set, view_set ? nsets : 0,
                                              reinterpret_cast<const float2 *>(pixelcoords), stream);
 }
+
+int mvp_raymarch_backward_deterministic(const mvp_backward_args *a, int64_t *acc_primpos, int64_t *acc_primrot, int64_t *acc_primscale,
+                                        int64_t *acc_tplate, uint32_t *det_max, const float *pixelcoords, const int32_t *view_set,
+                                        int32_t nsets, void *stream) {
+    if (!a) return MVP_ERR_NULL;
+    if (a->struct_size != sizeof(mvp_backward_args)) return MVP_ERR_STRUCT;
+    const int rc = view_set ? check_view_sets(a->shape, a->flags, view_set, nsets) : MVP_OK;
+    if (rc != MVP_OK) return rc;
+    DetBufs d;
+    d.acc[kDetTplate] = reinterpret_cast<long long *>(acc_tplate); d.acc[kDetPos] = reinterpret_cast<long long *>(acc_primpos);
+    d.acc[kDetRot] = reinterpret_cast<long long *>(acc_primrot); d.acc[kDetScale] = reinterpret_cast<long long *>(acc_primscale);
+    d.max = det_max;
+    return backward_impl(a, false, nullptr, nullptr, nullptr, view_set, view_set ? nsets : 0, reinterpret_cast<const float2 *>(pixelcoords),
+                         stream, &d);
+}
+
+#if defined(MVP_CPU_EMUL)
+// host mirror of the quantum rule, for the tests: the exponent of q for a tensor whose largest finite |value| has these fp32 bits
+int mvp_emul_det_quantum_exp(unsigned mbits) { return det_quantum_exp(mbits); }
+#endif
 
 #if defined(MVP_CPU_EMUL) && defined(MVP_EMUL_STATS)
 void mvp_emul_fwd_stats(long long *out) {

@@ -75,6 +75,7 @@ FLAG_TPLATE_BF16 = 8
 FLAG_GRAD_TPLATE_F32 = 16
 FLAG_NO_TPLATE_GRAD = 32
 FLAG_RAY_GRADS_ONLY = 64
+FLAG_DETERMINISTIC = 128
 FLAG_TEST_TINY_LISTS = 0x100
 ABI_VERSION = 8
 # layout pins, equal to the static_asserts in csrc/mvp_kernels.cu (tests/test_abi.py compares)
@@ -88,7 +89,8 @@ EXPORTS = ("mvp_abi_version", "mvp_build_config", "mvp_error_string", "mvp_works
            "mvp_compute_morton",
            "mvp_expand_views", "mvp_sum_views", "mvp_assemble_payload_forward_bf16", "mvp_assemble_payload_backward_bf16",
            "mvp_sum_views_bf16", "mvp_raymarch_backward_rays", "mvp_compute_raydirs_backward", "mvp_raymarch_forward_sets",
-           "mvp_raymarch_backward_sets", "mvp_raymarch_forward_pixels", "mvp_raymarch_backward_pixels", "mvp_debug_view_fallback_offset")
+           "mvp_raymarch_backward_sets", "mvp_raymarch_forward_pixels", "mvp_raymarch_backward_pixels", "mvp_debug_view_fallback_offset",
+           "mvp_raymarch_backward_deterministic")
 
 
 def _load():
@@ -135,6 +137,8 @@ def _load():
     lib.mvp_raymarch_forward_pixels.argtypes = [ctypes.POINTER(ForwardArgs), c_f, c_f, ctypes.c_int32, c_f]
     lib.mvp_raymarch_backward_pixels.restype = ctypes.c_int
     lib.mvp_raymarch_backward_pixels.argtypes = [ctypes.POINTER(BackwardArgs), c_f, c_f, ctypes.c_int32] + [c_f] * 4
+    lib.mvp_raymarch_backward_deterministic.restype = ctypes.c_int
+    lib.mvp_raymarch_backward_deterministic.argtypes = [ctypes.POINTER(BackwardArgs)] + [c_f] * 7 + [ctypes.c_int32, c_f]
     lib.mvp_compute_raydirs_backward.restype = ctypes.c_int
     lib.mvp_compute_raydirs_backward.argtypes = [ctypes.c_int32] * 3 + [c_f] * 5 + [ctypes.c_float] + [c_f] * 8
     lib.mvp_composite_forward.restype = ctypes.c_int
@@ -229,6 +233,13 @@ def require_camera_pixels():
     (mvp_raymarch_forward_pixels, mvp_raymarch_backward_pixels), which it reports as CAMERA_PIXELS=1 in its build configuration."""
     if "CAMERA_PIXELS=1" not in LIB.mvp_build_config().decode().split():
         raise RuntimeError("mvpraymarch_b200: this library (%s) does not generate camera rays at sample positions" % _build.LIB)
+
+
+def require_deterministic():
+    """Raise unless the library sums the primitive gradients in fixed point on request (mvp_raymarch_backward_deterministic,
+    MVP_FLAG_DETERMINISTIC), which it reports as DETERMINISTIC=1 in its build configuration."""
+    if "DETERMINISTIC=1" not in LIB.mvp_build_config().decode().split():
+        raise RuntimeError("mvpraymarch_b200: this library (%s) does not support deterministic gradients" % _build.LIB)
 
 
 def workspace_bytes(N, H, W, K, TD, TH, TW):

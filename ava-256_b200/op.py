@@ -84,6 +84,42 @@ def template_grad_dtype(dtype):
 
 _template_grad_block = template_grad_dtype     # for the functions whose keyword of the same name hides it
 
+_DETERMINISTIC = {}   # "on": the setting of the innermost active `deterministic_grads` context
+
+
+@contextlib.contextmanager
+def deterministic_grads(enabled=True):
+    """Within the block (enabled=True), raymarch calls return reproducible primitive gradients: the backward sums grad_primpos,
+    grad_primrot, grad_primscale and the template's gradient in 64-bit fixed point (C-ABI mvp_raymarch_backward_deterministic), so
+    two backwards of the same inputs give the same bits, whatever the order in which the GPU runs the warps, and the same sums
+    whatever the order of the views.  They agree with the default backward to within about 1e-6 of each tensor's largest entry;
+    images are unchanged.  The backward runs the render kernels twice (a pass that measures each tensor's range, then the
+    accumulating pass), and its int64 scratch is twice the size of the fp32 gradients (allocated by the forward for the gradients
+    autograd asks for, cleared by its render kernel).  Supported: algo 0, fp32 and bf16 templates (either `template_grad_dtype`),
+    per-view, shared and set primitives, usebvh=True, ray tensors, camera rays and pixelcoords, image planes.  Raises
+    NotImplementedError for algo 1 and for ray / camera gradients.  The decision is taken by the forward call and kept for its
+    backward.  The only way an unmodified caller of `mvpraymarch` opts in:
+
+        with ava256_b200.op.deterministic_grads():
+            rayrgba = mvpraymarch(raypos, raydir, stepsize, tminmax, primtransf, template, warp)
+        loss(rayrgba).backward()
+
+    `torch.use_deterministic_algorithms(True)` does not switch this on."""
+    prev = _DETERMINISTIC.get("on")
+    _DETERMINISTIC["on"] = bool(enabled)
+    try:
+        yield
+    finally:
+        _DETERMINISTIC["on"] = prev
+
+
+_deterministic_block = deterministic_grads     # for the functions whose keyword `deterministic` hides it
+
+
+def _det_context(deterministic):
+    """The `deterministic=` keyword of the entry points: None leaves the enclosing `deterministic_grads` setting."""
+    return contextlib.nullcontext() if deterministic is None else _deterministic_block(bool(deterministic))
+
 
 def _widen_bf16(t):
     """A bfloat16 tensor as fp32 (exact); anything else unchanged, so that other dtypes still meet the op's dtype check."""
@@ -113,6 +149,12 @@ def _grad_set(needs, first_prim, want_rays):
     if any(needs[first_prim:first_prim + 3]):
         return GRADS_NO_PAYLOAD
     return GRADS_RAYS_ONLY if want_rays else None
+
+
+def _empty_det_sums(gset, primpos, primrot, primscale, template):
+    """The deterministic backward's int64 sums of the set, one entry per gradient entry: [primpos, primrot, primscale, template, None]."""
+    e = lambda t: torch.empty(t.shape, dtype=torch.int64, device=t.device)  # noqa: E731
+    return [e(primpos), e(primrot), e(primscale), e(template) if gset == GRADS_ALL else None, None]
 
 
 def _empty_grads(gset, primpos, primrot, primscale, template, warp, usewarp, tflags):
@@ -147,6 +189,13 @@ class MVPRaymarch(Function):
         if options["usebvh"] is False:
             raise NotImplementedError("mvpraymarch_b200: usebvh=False passes a null BVH to the reference kernels "
                                       "(mvpraymarch.py:132-134) and is not a usable mode there either")
+        if options.get("_deterministic") and gradmode and any(ctx.needs_input_grad):
+            if algo == 1:
+                raise NotImplementedError("mvpraymarch_b200: deterministic gradients need algo 0 (the warp field's gradient is "
+                                          "summed with float atomics)")
+            if options.get("_ray_grads") and any(ctx.needs_input_grad[i] for i in ray_inputs):
+                raise NotImplementedError("mvpraymarch_b200: deterministic gradients of rays and cameras are not supported (their "
+                                          "per-ray sums use shared-memory float atomics)")
         camera = options.get("_camera")        # (viewpos, viewrot, focal, princpt, volradius, H, W): rays generated in the kernels
         pixels = options.get("_pixels")        # with a camera: [N,H,W,2] sample positions of its rays, or None (the integer grid)
         if camera is not None:
@@ -190,6 +239,9 @@ class MVPRaymarch(Function):
                 _lib.require_grad_select()
         grad_f32 = bf16 and _check_template_grad_dtype(options.get("_template_grad_dtype")) is torch.float32 and gset == GRADS_ALL
         tflags = _lib.tplate_flags(bf16, grad_f32)                     # + MVP_FLAG_GRAD_TPLATE_F32: fp32 template gradient
+        det = bool(options.get("_deterministic")) and gradmode         # fixed-point primitive gradients (deterministic_grads)
+        if det:
+            _lib.require_deterministic()
         if warp is not None:                                           # mvpraymarch.py:124
             assert warp.is_contiguous() and warp.dim() == 6 and warp.size(-1) == 3, \
                 "channels-last warp field [N,K,WD,WH,WW,3] required"
@@ -240,7 +292,8 @@ class MVPRaymarch(Function):
             a = _lib.ForwardArgs()
             a.shape = _lib.Shape(N, H, W, K, TD, TH, TW)
             a.stepsize, a.fadescale, a.fadeexp = float(stepsize), float(options["fadescale"]), float(options["fadeexp"])
-            a.flags = (_lib.FLAG_SHARED_PRIMS if shared else 0) | tflags | _GRAD_SET_FLAGS.get(gset, 0)
+            a.flags = (_lib.FLAG_SHARED_PRIMS if shared else 0) | tflags | _GRAD_SET_FLAGS.get(gset, 0) | \
+                (_lib.FLAG_DETERMINISTIC if det else 0)
             a.raypos, a.raydir, a.tminmax = _ptr(raypos), _ptr(raydir), _ptr(tminmax)
             if camera is not None:
                 a.camera = _lib.Camera(_ptr(viewpos), _ptr(viewrot), _ptr(focal), _ptr(princpt), float(volradius), 0)
@@ -263,7 +316,10 @@ class MVPRaymarch(Function):
                 # The gradient buffers of the backward (mvpraymarch.py:240-246 zeros_like's them there) are made now and zero-filled
                 # by the forward's render kernel on the side (mvp_forward_args::clear_grad_*): no memset pass in the step.  Only
                 # those of the gradient set: a frozen template costs no template-sized buffer.
-                grads = _empty_grads(gset, primpos, primrot, primscale, template, warp, usewarp, tflags)
+                # Deterministic: the int64 sums of the set take their place, and the gradients are allocated by the backward,
+                # which writes them.
+                grads = _empty_det_sums(gset, primpos, primrot, primscale, template) if det else \
+                    _empty_grads(gset, primpos, primrot, primscale, template, warp, usewarp, tflags)
                 a.clear_grad_primpos, a.clear_grad_primrot, a.clear_grad_primscale = _ptr(grads[0]), _ptr(grads[1]), _ptr(grads[2])
                 a.clear_grad_tplate, a.clear_grad_warp = _ptr(grads[3]), _ptr(grads[4])
             stream = torch.cuda.current_stream(dev).cuda_stream
@@ -287,6 +343,7 @@ class MVPRaymarch(Function):
             ctx.shared = shared
             ctx.view_set = view_set
             ctx.tflags = tflags
+            ctx.det = det
         if planes:
             return rayrgb, rayalpha
         return rayrgba
@@ -326,8 +383,15 @@ def _march_backward(ctx, grad_rayrgba, grad_rayalpha, want_rays):
         if gset == GRADS_RAYS_ONLY:
             assert want_rays, "a rays-only backward without ray gradients"
         grads, ctx.grads = ctx.grads, None
-        fresh = grads is not None          # the forward's render kernel zero-filled them; a second backward through the
-        if not fresh:                      # same graph (retain_graph) gets new ones, zero-filled by the library
+        # the forward's render kernel zero-filled them; a second backward through the same graph (retain_graph) gets new ones,
+        # zero-filled by the library.  Deterministic: those buffers are the int64 sums, and the gradients are written by the library.
+        fresh = grads is not None
+        det = ctx.det
+        sums = None
+        if det:
+            sums = grads if fresh else _empty_det_sums(gset, primpos, primrot, primscale, template)
+            grads = _empty_grads(gset, primpos, primrot, primscale, template, warp, usewarp, ctx.tflags)
+        elif not fresh:
             grads = _empty_grads(gset, primpos, primrot, primscale, template, warp, usewarp, ctx.tflags)
         grad_primpos, grad_primrot, grad_primscale, grad_template, grad_warp = grads
         if warp is not None and not usewarp and gset == GRADS_ALL:  # mvpraymarch.py:246 (zero when algo 0 ignores it)
@@ -362,6 +426,11 @@ def _march_backward(ctx, grad_rayrgba, grad_rayalpha, want_rays):
             # written for every ray by the library: no zero-fill
             rays = (torch.empty((N, H, W, 3), device=dev), torch.empty((N, H, W, 3), device=dev), torch.empty((N, H, W, 2), device=dev))
         pixels = options.get("_pixels")
+        if det:
+            det_max = torch.empty(4, dtype=torch.int32, device=dev)
+            _lib.check(_lib.LIB.mvp_raymarch_backward_deterministic(ctypes.byref(a), *(_ptr(t) for t in sums[:4]), _ptr(det_max),
+                                                                    _ptr(pixels), _ptr(ctx.view_set), primpos.size(0), stream))
+            return (grad_primpos, grad_primrot, grad_primscale, grad_template, grad_warp), None
         if pixels is not None and want_rays:
             # The ray-gradient backward of a pixels forward marches the rays mvp_compute_raydirs makes from the same pixelcoords:
             # bit for bit the rays the forward generated, so its acceleration structure and saved tile lists hold for them.  The
@@ -530,6 +599,7 @@ def mvpraymarch(
         "maxhitboxes": maxhitboxes, "synchitboxes": synchitboxes, "chlast": chlast, "fadescale": fadescale,
         "fadeexp": fadeexp, "accum": accum, "termthresh": termthresh, "griddim": griddim, "blocksize": blocksize,
         "bwdblocksize": bwdblocksize, "_order": order, "_template_grad_dtype": _TEMPLATE_GRAD.get("dtype"),
+        "_deterministic": bool(_DETERMINISTIC.get("on")),
     }
     if _VIEW_SET.get("map") is not None:
         options["_view_set"] = _VIEW_SET["map"]
@@ -595,7 +665,7 @@ def _view_set_tensor(view_set, N, S, dev):
 
 
 def mvpraymarch_sets(raypos, raydir, stepsize, tminmax, primtransf, template, warp, view_set, planes=False, template_grad_dtype=None,
-                     **kwargs):
+                     deterministic=None, **kwargs):
     """`mvpraymarch` over S primitive sets -- S subjects, or S frames -- rendered in one launch, view n from set view_set[n]: the
     primitives (primtransf, template, warp) are [S,K,...] with 1 <= S <= N, and so are their gradients (the template's in its dtype,
     or fp32 per `template_grad_dtype`).  Each set's gradient sums those of its views; a set no view shows gets zero gradients.
@@ -604,14 +674,15 @@ def mvpraymarch_sets(raypos, raydir, stepsize, tminmax, primtransf, template, wa
     renders empty (zero colour and alpha) and contributes no gradient.  Replaces `payload.expand_views` + `mvpraymarch` +
     `sum_views` for views that share a subject: no per-view copy of the primitives and no per-view gradient.  With usebvh=True each
     set is marched in its own Morton order.  The other keyword arguments are those of `mvpraymarch`; ray gradients (camera fitting)
-    come through `mvpraymarch_camera(..., view_set=...)`.
+    come through `mvpraymarch_camera(..., view_set=...)`.  deterministic=True: reproducible primitive gradients (see
+    `deterministic_grads`); None leaves the setting of an enclosing `deterministic_grads` block.
     Returns rayrgba [N,H,W,4], or (rayrgb [N,3,H,W], rayalpha [N,1,H,W]) with planes=True."""
     if view_set is None:
         raise TypeError("mvpraymarch_sets: view_set is required (use mvpraymarch for per-view or shared primitives)")
     march = mvpraymarch_planes if planes else mvpraymarch
     grad_block = _template_grad_block(template_grad_dtype) if _check_template_grad_dtype(template_grad_dtype) is not None \
         else contextlib.nullcontext()
-    with grad_block, _view_set_block(view_set):
+    with grad_block, _view_set_block(view_set), _det_context(deterministic):
         return march(raypos, raydir, stepsize, tminmax, primtransf, template, warp, **kwargs)
 
 
@@ -626,7 +697,7 @@ def mvpraymarch_planes(*args, **kwargs):
 
 
 def mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, volradius, stepsize, primtransf, template, warp, planes=False,
-                       camera_grad=False, template_grad_dtype=None, view_set=None, **kwargs):
+                       camera_grad=False, template_grad_dtype=None, view_set=None, deterministic=None, **kwargs):
     """`compute_raydirs` + `mvpraymarch` of models/autoencoder.py:240-252 as ONE call: the first six parameters are those of the
     reference's compute_raydirs (extensions/utils/utils.py:48-51), the rest those of `mvpraymarch` after its ray arguments.
 
@@ -650,7 +721,14 @@ def mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, volradius,
     template_grad_dtype=torch.float32 accumulates a bfloat16 template's gradient in fp32 (see the `template_grad_dtype` context
     manager); None leaves the setting of an enclosing `template_grad_dtype` block, by default the template's own dtype.
     view_set: the views render S primitive sets [S,K,...], view n set view_set[n] (see `mvpraymarch_sets`).
+    deterministic=True: reproducible primitive gradients (see `deterministic_grads`; not with camera_grad); None leaves the setting
+    of an enclosing `deterministic_grads` block.
     Returns rayrgba [N,H,W,4], or (rayrgb [N,3,H,W], rayalpha [N,1,H,W]) with planes=True."""
+    if deterministic is not None:
+        with _deterministic_block(bool(deterministic)):
+            return mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, volradius, stepsize, primtransf, template, warp,
+                                      planes=planes, camera_grad=camera_grad, template_grad_dtype=template_grad_dtype,
+                                      view_set=view_set, **kwargs)
     if view_set is not None:
         with _view_set_block(view_set):
             return mvpraymarch_camera(viewpos, viewrot, focal, princpt, pixelcoords, volradius, stepsize, primtransf, template, warp,

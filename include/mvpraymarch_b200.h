@@ -104,6 +104,10 @@ typedef struct mvp_shape {
                                  * clear_grad_*): they may be NULL and are ignored.  The backward skips the payload scatter and the
                                  * transform-gradient sums.  mvp_raymarch_backward with this flag returns MVP_ERR_NULL: it would have
                                  * no output.  MVP_FLAG_ZERO_GRADS zero-fills only the buffers a call's flags request. */
+#define MVP_FLAG_DETERMINISTIC 128u /* forward: the clear_grad_primpos / primrot / primscale / tplate buffers are the int64 sums of the
+                                 * mvp_raymarch_backward_deterministic call that follows (8 bytes per entry, four entries per voxel
+                                 * whatever the template's type) and are cleared as such.  The backward ignores the bit: the entry
+                                 * point chooses the mode.  The library supports it iff mvp_build_config() lists DETERMINISTIC=1. */
 #define MVP_FLAG_TEST_TINY_LISTS 0x100u /* test hook: forward keeps at most 16 saved tile-list entries per view, so almost
                                  * every tile takes the backward's rebuild path */
 
@@ -263,6 +267,31 @@ int mvp_raymarch_forward_pixels(const mvp_forward_args *args, const float *pixel
                                 void *stream);
 int mvp_raymarch_backward_pixels(const mvp_backward_args *args, const float *pixelcoords, const int32_t *view_set, int32_t nsets,
                                  float *grad_raypos, float *grad_raydir, float *grad_tminmax, void *stream);
+
+/* Reproducible primitive gradients: mvp_raymarch_backward with grad_primpos / primrot / primscale / tplate summed in 64-bit two's-
+ * complement fixed point, so that they depend only on the inputs -- not on the order in which warps are scheduled, on which tiles
+ * the 512-entry kernels take, or on the order of the views.  The images of the forward are unchanged.
+ *   - The backward runs twice.  The measure pass finds, per gradient tensor, the largest |value| M that goes into one reduction (a
+ *     merged voxel group's payload sum, or a warp's transform sum over one slab visit); the tensor's quantum is q = 2^(e - 38) with
+ *     2^e the smallest power of two >= M (q >= 2^-126).  The accumulate pass adds llrint(value / q) to the int64 sums with integer
+ *     reductions, and a conversion writes (float)sum * q into the gradient buffers, which are WRITTEN, not accumulated into (a bf16
+ *     template gradient rounded once more, to nearest even).
+ *   - Limits: an entry must take fewer than 2^24 reductions (every term is at most 2^38 in magnitude); the result keeps 38 bits
+ *     below the tensor's largest reduction, so an entry far smaller than that loses relative precision.
+ *   - An entry that received a non-finite value comes out NaN, and no other entry does.
+ *   - acc_primpos [nsets,K,3], acc_primrot [nsets,K,9], acc_primscale [nsets,K,3], acc_tplate [nsets,K,TD,TH,TW,4] (NULL with
+ *     MVP_FLAG_NO_TPLATE_GRAD): caller-owned int64 scratch, 8-byte aligned, zero on entry -- cleared by the gradient-mode forward
+ *     called with MVP_FLAG_DETERMINISTIC and these buffers as clear_grad_*, or by MVP_FLAG_ZERO_GRADS here.  nsets is N per view,
+ *     1 with MVP_FLAG_SHARED_PRIMS, or the sets call's nsets.  det_max: caller-owned uint32 [4] (4-byte aligned), written.
+ *   - pixelcoords: NULL, or the pixels form of mvp_raymarch_backward_pixels; view_set: NULL, or the sets form with the rules and
+ *     argument errors of mvp_raymarch_backward_sets.  Per-view, shared and set primitives, Morton `order`, camera rays, image
+ *     planes, fp32 and bf16 templates (MVP_FLAG_GRAD_TPLATE_F32 included) and MVP_FLAG_NO_TPLATE_GRAD are supported.
+ *   - algo 1 is MVP_ERR_ALGO; MVP_FLAG_RAY_GRADS_ONLY is MVP_ERR_NULL (this entry point computes no ray gradients).
+ * It launches the render kernels twice and one conversion kernel per gradient tensor.  Argument errors are returned before any
+ * device work.  The library supports it iff mvp_build_config() lists DETERMINISTIC=1. */
+int mvp_raymarch_backward_deterministic(const mvp_backward_args *args, int64_t *acc_primpos, int64_t *acc_primrot, int64_t *acc_primscale,
+                                        int64_t *acc_tplate, uint32_t *det_max, const float *pixelcoords, const int32_t *view_set,
+                                        int32_t nsets, void *stream);
 
 /* Pinhole ray generation + unit-cube clip (reference: extensions/utils/utils_kernel.cu:12-52).
  * viewpos [N,3], viewrot [N,3,3], focal [N,2], princpt [N,2], pixelcoords [N,H,W,2] or NULL (integer grid);
